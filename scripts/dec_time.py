@@ -1,10 +1,17 @@
-"""Time only the decoder section of the C2 step (quick A/B of decoder variants)."""
-import os, sys, statistics
+"""Time only the decoder section of the C2 step (quick A/B of decoder variants).
+
+    TACO_TRACE=1 python scripts/dec_time.py [--precision fp32x3|tf32|fp32]
+
+With TACO_TRACE set, the traced kernel instantiation also records per-slot and per-phase clocks of CTA 0."""
+import argparse, os, sys, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from tacotron_b200 import Config, Tacotron
+ap = argparse.ArgumentParser()
+ap.add_argument("--precision", default="fp32x3", choices=["fp32x3", "tf32", "fp32"], help="default: the benchmark's mode")
+args = ap.parse_args()
 B, TX, T, R = 32, 128, 200, 5
-m = Tacotron(Config(r=R, vocab_size=64, max_decode_iter=T, precision="tf32"), None, train=False, seed=1)
+m = Tacotron(Config(r=R, vocab_size=64, max_decode_iter=T, precision=args.precision), None, train=False, seed=1)
 g = torch.Generator().manual_seed(0)
 inp = {"text": torch.randint(1, 64, (B, TX), generator=g, dtype=torch.int32).cuda(), "text_length": torch.full((B,), TX, dtype=torch.int32).cuda()}
 m.step_ns = torch.zeros(T, dtype=torch.int64, device="cuda")
@@ -18,7 +25,7 @@ for _ in range(5):
     tt = dict(m._marks); m._marks = None
     dec.append(tt["encoder"].elapsed_time(tt["decoder"]))
 ns = m.step_ns.cpu().numpy()
-print("LL mode", os.environ.get("TACO_DEC_LL", "default"), "decoder ms", statistics.median(dec), "step p50 us", float(statistics.median(((ns[1:]-ns[:-1])/1e3).tolist())))
+print("precision", args.precision, "decoder ms", statistics.median(dec), "step p50 us", float(statistics.median(((ns[1:]-ns[:-1])/1e3).tolist())))
 if os.environ.get("TACO_TRACE"):
     import numpy as np
     ws = m.runtime.dec_ws.view(torch.int64).cpu().numpy()
@@ -33,15 +40,17 @@ if os.environ.get("TACO_TRACE"):
     print("per-slot median ns (CTA 0):", {n_: int(v) for n_, v in zip(names, med)}, "sum", int(med.sum()))
     ck = ws[total + 16 * T + 16: total + 16 * T + 16 + 4 * 20 * 8].reshape(4, 20, 8)
     inames = ["IN", "G1", "C1", "G2", "C2", "G3", "C3", "OQP", "AP2"]
-    print("stage: start->on-chain loads issued | (off-chain half) ->on-chain weights | ->mma done | (finish) ->partials | ->sync | ->epilogue   [cycles, CTA0 thread0, step 11]")
-    st = 1
+    print("stage: start->on-chain loads issued | (off-chain half) ->on-chain weights | ->mma done | (finish) ->partials | ->sync | ->epilogue"
+          "   [cycles, CTA0 thread0, median of steps 10..12]")
     for i, nm in enumerate(inames):
-        c = ck[st, i]
-        if c[3] == 0: continue
-        f = lambda a, b: int(c[a] - c[b]) if c[a] and c[b] else -1
-        nxt = ck[st, i + 1, 3] if i + 1 < len(inames) else ck[st + 1, 0, 3]
-        print(f"  {nm:8s} {f(0,3):6d} {f(1,0):6d} {f(2,1):6d} | {f(4,2):6d} {f(5,4):6d} {f(6,5):6d} | total {int(nxt - c[3]):6d}")
-    c = ck[1, 8]      # A|P2 stage record of step 11: attention on warp 0 / thread 0
-    if c[3]:
+        if ck[1, i, 3] == 0: continue
+        def f(a, b):
+            v = [int(ck[st, i, a] - ck[st, i, b]) for st in range(3) if ck[st, i, a] and ck[st, i, b]]
+            return int(statistics.median(v)) if v else -1
+        nxt = [ck[st, i + 1, 3] if i + 1 < len(inames) else ck[st + 1, 0, 3] for st in range(3)]
+        total = int(statistics.median([int(nxt[st] - ck[st, i, 3]) for st in range(3)]))
+        print(f"  {nm:8s} {f(0,3):6d} {f(1,0):6d} {f(2,1):6d} | {f(4,2):6d} {f(5,4):6d} {f(6,5):6d} | total {total:6d}")
+    c = ck[:3, 8]     # A|P2 stage records: attention on warp 0 / thread 0
+    if c[1, 3]:
         print("attention (cycles from slot start): q arrived+exp %d | bar1 %d | scores %d | bar2 %d | stats+bar3 %d | ctx partial+push %d | merged ctx stored %d"
-              % tuple(int(c[i] - c[3]) for i in (0, 1, 2, 4, 5, 6, 7)))
+              % tuple(int(statistics.median([int(c[st, i] - c[st, 3]) for st in range(3)])) for i in (0, 1, 2, 4, 5, 6, 7)))

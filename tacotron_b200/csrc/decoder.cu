@@ -31,14 +31,18 @@
 //     registers; only K=256 (16 KB of operand words per CTA) is ingested on the chain.
 //   * on-chain weight slices are resident in shared memory (124 KB); the off-chain slices (and, when the keys/values
 //     leave too little shared memory, further slices) are read every step from the packed buffer in global memory,
-//     which stays in the 50 MB L2.  Their loads are issued together with the operand loads of the same half, so they
-//     travel in the shadow of the previous slot's exchange.
+//     which stays in the 50 MB L2.  They are loaded one stage early, together with the off-chain operand words, so
+//     they travel while the previous stage's epilogue runs (loaded at the start of their own stage, their L2 latency
+//     made the off-chain half ~400 cycles longer than the on-chain operand's hop on an H100, so it sat on the chain).
+//     Only IN, the first stage of a step, loads them in place.
 //   * MMA orientation swapped: M = 16 weight columns of the CTA's slice, N = the 8 utterance rows of the CTA's row
 //     group, so the 16-column gate stage has no zero-padded rows (half the MMAs of v3).
 //   * attention: the four CTAs that share an utterance (blockIdx / 4) each score a quarter of the memory; partial softmax
 //     statistics and partial contexts are exchanged as {value,tag} words through a small per-utterance region of the
 //     workspace (L2), each CTA normalises and publishes 64 context columns and its own alignment slice: the consumer
-//     ingests 256 context words per row instead of 4 x 256 partials + statistics.  (No thread-block cluster:
+//     ingests 256 context words per row instead of 4 x 256 partials + statistics.  A merging thread requests all of its
+//     words (each quarter's adjacent {max, sum} pair with one 16-byte load, its four context partials) before it checks
+//     any tag: one L2 round trip on the chain instead of twelve dependent ones.  (No thread-block cluster:
 //     cudaOccupancyMaxActiveClusters reported 30 co-resident clusters of four such CTAs on the H100 80GB HBM3 this was
 //     built on, fewer than the 32 this grid needs; the count depends on each die's GPC configuration.)
 //     tanh(k+q) = 1 - 2/(e^{2k} e^{2q} + 1) with e^{2k} precomputed once and e^{2q} once per step: one MUFU per
@@ -167,14 +171,18 @@ __device__ __forceinline__ float2 ll_wait2(const uint64_t* p, uint32_t tag) {
     ll_spin(v, p, tag);
     return make_float2(__uint_as_float((uint32_t)v.x), __uint_as_float((uint32_t)v.y));
 }
-// one {value, tag} word (the attention exchange between the four CTAs of an utterance)
-__device__ __forceinline__ float ll_wait1(const uint64_t* p, uint32_t tag) {
+// one {value, tag} word (the attention exchange between the four CTAs of an utterance).  The first load is issued apart
+// from the tag check so that a thread can have all the words it needs in flight before it waits for any of them.
+__device__ __forceinline__ uint64_t ll_load1(const uint64_t* p) {
     uint64_t v;
+    asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ float ll_spin1(uint64_t& v, const uint64_t* p, uint32_t tag) {
     uint32_t spins = 0;
-    while (true) {
-        asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-        if ((uint32_t)(v >> 32) == tag) break;
+    while ((uint32_t)(v >> 32) != tag) {
         if (++spins > (1u << 24)) __trap();
+        v = ll_load1(p);
     }
     return __uint_as_float((uint32_t)v);
 }
@@ -241,21 +249,25 @@ __device__ __forceinline__ const float* weight_ptr(uint32_t ww, const float* res
 __device__ __forceinline__ uint32_t seg_word(const SegDesc& d, int cs) {
     return d.smem_off >= 0 ? (uint32_t)d.smem_off : (0x80000000u | (uint32_t)(d.g_off + (int64_t)cs * d.slice_floats));
 }
-template <int FL, int MT, int NS_, bool TR>
-__device__ __forceinline__ void consume(float (&acc)[2][3][4], ulonglong2 (&v)[4], const uint64_t* p0, int nkt, int widx, int nw, int s0,
-                                        uint32_t tag, uint32_t w1, uint32_t w2, int wslot, const float* res_s, const float* packed,
-                                        int lane, long long* ck) {
-    float w[MT][NS_ * FL];
-    __syncwarp();
+// weight fragments of one call -> w[(mt * NS_ + i) * FL ..] (tile mt, slot i); w may be longer than MT * NS_ * FL
+template <int FL, int MT, int NS_, int N>
+__device__ __forceinline__ void load_weights(float (&w)[N], uint32_t w1, uint32_t w2, int wslot, const float* res_s, const float* packed, int lane) {
+    static_assert(N >= MT * NS_ * FL, "weight fragment array too short");
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
         const float* wp = weight_ptr(mt ? w2 : w1, res_s, packed) + ((size_t)wslot * 32 + lane) * FL;
+        float* wm = w + mt * NS_ * FL;
 #pragma unroll
         for (int i = 0; i < NS_; ++i) {
-            if constexpr (FL == 4) { const float4 t = *reinterpret_cast<const float4*>(wp + (size_t)i * 32 * FL); w[mt][4 * i] = t.x; w[mt][4 * i + 1] = t.y; w[mt][4 * i + 2] = t.z; w[mt][4 * i + 3] = t.w; }
-            else                   { const float2 t = *reinterpret_cast<const float2*>(wp + (size_t)i * 32 * FL); w[mt][2 * i] = t.x; w[mt][2 * i + 1] = t.y; }
+            if constexpr (FL == 4) { const float4 t = *reinterpret_cast<const float4*>(wp + (size_t)i * 32 * FL); wm[4 * i] = t.x; wm[4 * i + 1] = t.y; wm[4 * i + 2] = t.z; wm[4 * i + 3] = t.w; }
+            else                   { const float2 t = *reinterpret_cast<const float2*>(wp + (size_t)i * 32 * FL); wm[2 * i] = t.x; wm[2 * i + 1] = t.y; }
         }
     }
+}
+// wait for the operand words v (loads already in flight) and multiply them into acc with weight fragments w (load_weights order)
+template <int FL, int MT, int NS_, bool TR, int N>
+__device__ __forceinline__ void multiply(float (&acc)[2][3][4], ulonglong2 (&v)[4], const float (&w)[N], const uint64_t* p0, int nkt, int widx,
+                                         int nw, int s0, uint32_t tag, long long* ck) {
     if (TR && ck) ck[1] = clock64();
 #pragma unroll
     for (int i = 0; i < NS_; ++i) {
@@ -266,10 +278,19 @@ __device__ __forceinline__ void consume(float (&acc)[2][3][4], ulonglong2 (&v)[4
             split_tf32(__uint_as_float((uint32_t)v[i].y), bh1, bl1);
             __syncwarp();                               // lanes arrive from divergent polling loops
 #pragma unroll
-            for (int mt = 0; mt < MT; ++mt) ktile_mma<FL>(acc[mt], bh0, bl0, bh1, bl1, &w[mt][i * FL]);
+            for (int mt = 0; mt < MT; ++mt) ktile_mma<FL>(acc[mt], bh0, bl0, bh1, bl1, &w[(mt * NS_ + i) * FL]);
         }
     }
     if (TR && ck) ck[2] = clock64();
+}
+template <int FL, int MT, int NS_, bool TR>
+__device__ __forceinline__ void consume(float (&acc)[2][3][4], ulonglong2 (&v)[4], const uint64_t* p0, int nkt, int widx, int nw, int s0,
+                                        uint32_t tag, uint32_t w1, uint32_t w2, int wslot, const float* res_s, const float* packed,
+                                        int lane, long long* ck) {
+    float w[MT * NS_ * FL];
+    __syncwarp();
+    load_weights<FL, MT, NS_>(w, w1, w2, wslot, res_s, packed, lane);
+    multiply<FL, MT, NS_, TR>(acc, v, w, p0, nkt, widx, nw, s0, tag, ck);
 }
 
 struct ItemRec { uint32_t flags, pre_base; int pre_tagd; uint32_t pre_w; uint32_t on_base; int on_tagd; uint32_t on_w1, on_w2; int on_nkt, pad0, pad1, pad2; };   // 48 bytes, in smem
@@ -555,13 +576,29 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
         }
         if (TR && cktr) cktr[6] = clock64();
         if (tid >= 128) return;
-        // merge: global max / sum from the four quarter statistics
+        // merge: global max / sum from the four quarter statistics.  Every exchange word this thread needs ({max, sum} of
+        // each quarter: one 16-byte load; its context partials) is requested before any tag is checked, so the merge waits
+        // for one L2 round trip instead of one per word; only words that were not yet published are polled again.
+        const uint64_t* xs = xstat + xp * 4 * 2;
+        const uint64_t* xc = xctx + xp * 4 * ENC + 64 * aq + tid;
+        ulonglong2 sw[4];
+        uint64_t cw[4];
+#pragma unroll
+        for (int qd = 0; qd < 4; ++qd) sw[qd] = ll_load2(xs + qd * 2);
+        if (tid < 64) {
+#pragma unroll
+            for (int qd = 0; qd < 4; ++qd) cw[qd] = ll_load1(xc + qd * ENC);
+        }
         float mq[4], wq[4], M = -INFINITY, S = 0.f, w_own = 0.f;
 #pragma unroll
-        for (int qd = 0; qd < 4; ++qd) { mq[qd] = ll_wait1(xstat + (xp * 4 + qd) * 2, tag); M = fmaxf(M, mq[qd]); }
+        for (int qd = 0; qd < 4; ++qd) {
+            ll_spin(sw[qd], xs + qd * 2, tag);
+            mq[qd] = __uint_as_float((uint32_t)sw[qd].x);
+            M = fmaxf(M, mq[qd]);
+        }
 #pragma unroll
         for (int qd = 0; qd < 4; ++qd) {
-            const float sq = ll_wait1(xstat + (xp * 4 + qd) * 2 + 1, tag);
+            const float sq = __uint_as_float((uint32_t)sw[qd].y);
             wq[qd] = (mq[qd] == -INFINITY) ? 0.f : __expf(mq[qd] - M);
             S = fmaf(wq[qd], sq, S);
             if (qd == (int)aq) w_own = wq[qd];
@@ -570,7 +607,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
         if (tid < 64) {                                  // final context column 64 aq + tid  (tag of the step that consumes it)
             float c = 0.f;
 #pragma unroll
-            for (int qd = 0; qd < 4; ++qd) c = fmaf(wq[qd], ll_wait1(xctx + (xp * 4 + qd) * ENC + 64 * aq + tid, tag), c);
+            for (int qd = 0; qd < 4; ++qd) c = fmaf(wq[qd], ll_spin1(cw[qd], xc + qd * ENC, tag), c);
             ll_store(ctx_out, c * inv, tag + 1);
             if (TR && cktr) cktr[7] = clock64();
         } else {                                         // alignments of this quarter (AttentionWrapper alignment_history)
@@ -715,7 +752,12 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     const int n_items = P.n_items;
     const uint32_t itab_a = smem_u32(itab);
     ulonglong2 vp[4];                                   // operand words of the off-chain half (prefetched one finish() early)
-    bool pref = false;                                  // vp[] already holds the loads of the current stage's off-chain half
+    float wpre[8];                                      // and its weight fragments (FL = 4: 2 slots x 4 floats; FL = 2: the first 4)
+    bool pref = false;                                  // vp[] / wpre[] already hold the loads of the current stage's off-chain half
+    auto load_pre_weights = [&](int knd, uint32_t ww) {
+        if (knd == IK_F4) load_weights<4, 1, 2>(wpre, ww, 0u, warp * 2, res_s, packed, lane);
+        else              load_weights<2, 1, 2>(wpre, ww, 0u, warp * 2, res_s, packed, lane);
+    };
     auto ld_rec = [&](int ii, uint4& r0, uint4& r1, uint32_t& nkt) {
         asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r0.x), "=r"(r0.y), "=r"(r0.z), "=r"(r0.w) : "r"(itab_a + ii * 48));
         asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r1.x), "=r"(r1.y), "=r"(r1.z), "=r"(r1.w) : "r"(itab_a + ii * 48 + 16));
@@ -752,24 +794,29 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             const bool has_pre = ((r0.x >> 16) & 1) && !(t == 0 && ((r0.x >> 17) & 1));
             const uint64_t* ppre = ws + r0.y + warp * 64 + lane_w;
             const uint32_t ptag = (uint32_t)(t + (int)r0.z), otag = (uint32_t)(t + (int)r1.y);
-            if (has_pre && !pref) issue_loads<2>(vp, ppre, 32, warp, NWARP, 0);
+            if (has_pre && !pref) {
+                issue_loads<2>(vp, ppre, 32, warp, NWARP, 0);
+                __syncwarp();
+                load_pre_weights(kind, r0.w);
+            }
             if (kind == IK_F4) {
-                if (has_pre) consume<4, 1, 2, false>(acc, vp, ppre, 32, warp, NWARP, 0, ptag, r0.w, 0u, warp * 2, res_s, packed, lane, nullptr);
+                if (has_pre) multiply<4, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
                 consume<4, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
             } else if (kind == IK_F2) {
-                if (has_pre) consume<2, 1, 2, false>(acc, vp, ppre, 32, warp, NWARP, 0, ptag, r0.w, 0u, warp * 2, res_s, packed, lane, nullptr);
+                if (has_pre) multiply<2, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
                 consume<2, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
             } else if (kind == IK_F2CP) {
-                if (has_pre) consume<2, 1, 2, false>(acc, vp, ppre, 32, warp, NWARP, 0, ptag, r0.w, 0u, warp * 2, res_s, packed, lane, nullptr);
+                if (has_pre) multiply<2, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
                 consume<2, 1, 3, TR>(acc, v, pon, 48, warp, NWARP, s0, otag, r1.z, 0u, warp * 3, res_s, packed, lane, ck);
             } else {
                 consume<4, 2, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, r1.w, warp * 2, res_s, packed, lane, ck);
             }
             pref = false;
-            // the next stage's off-chain operand is already known: put its loads in flight now, they travel while this
-            // stage's epilogue runs
+            // the next stage's off-chain operand is already known: put its loads in flight now, together with those of its
+            // weight fragments; they travel while this stage's epilogue runs
             if (ii + 1 < n_items && ((nr0.x >> 16) & 1)) {
                 issue_loads<2>(vp, ws + nr0.y + warp * 64 + lane_w, 32, warp, NWARP, 0);
+                load_pre_weights(nr0.x & 0xff, nr0.w);
                 pref = true;
             }
             finish(stage, t);
