@@ -55,7 +55,8 @@ int         taco_device_info(int* sm_count, int* cc_major, int* cc_minor);
  *   residual add               models/ops.py:92
  *   highway gate               models/ops.py:32-45 (TACO_EPI_HIGHWAY)
  * Y[b,t,n] = epi( sum_{j<taps} sum_{c<C} X[b, t+tap0+j, c] * W[j,c,n] ),  zero outside [0,T).
- * epi(v) = (act(v + bias[n]) * scale[n] + shift[n]) * keep[b,t,n]*keep_scale + residual[b,t,n]
+ * epi(v) = (act(v + bias[n] + bias_utt[b*ldbu + n]) * scale[n] + shift[n]) * keep[b,t,n]*keep_scale + residual[b,t,n]
+ * (bias_utt: a per-utterance bias, e.g. a speaker-dependent term; the two biases are added to each other first)
  * Bank mode (bank_K > 0): N = bank_K*bank_cout; output columns [(k-1)*cout, k*cout) come from
  * filter k (k taps, tap0 = -(k-1)/2).  W then points at the K filters stored back to back
  * (W1 [1][C][cout], W2 [2][C][cout], ...), Wp at the packed form made by taco_pack_weight.
@@ -88,6 +89,8 @@ typedef struct taco_linear_desc {
     int32_t        pool;     /* 1: fuse max_pooling1d(2,1,'same') over t after the affine    */
                              /*    (models/ops.py:66-71); tensor-core path only              */
     int32_t        impl;     /* TACO_IMPL_*                                                  */
+    const float*   bias_utt; /* [B][ldbu] per-utterance bias or NULL; not with TACO_EPI_HIGHWAY */
+    int64_t        ldbu;
 } taco_linear_desc;
 
 int taco_linear_fwd(const taco_linear_desc* d, void* stream);
@@ -126,6 +129,11 @@ int taco_mask_rows(const float* X, const int32_t* length, float* Y, int B, int T
 int taco_bigru_fwd(const float* xp, const float* Wg_h_fw, const float* Wc_h_fw,
                    const float* Wg_h_bw, const float* Wc_h_bw,
                    float* out, int B, int T, void* stream);
+/* same, with initial states h0_fw / h0_bw [B][128] (NULL = zero state; initial_state_fw/bw of
+ * bidirectional_dynamic_rnn, models/ops.py:111-126: the speaker-dependent state of a multi-speaker model) */
+int taco_bigru_fwd_h0(const float* xp, const float* Wg_h_fw, const float* Wc_h_fw,
+                      const float* Wg_h_bw, const float* Wc_h_bw, const float* h0_fw, const float* h0_bw,
+                      float* out, int B, int T, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Decoder: tacotron.py:46-105 create_decoder + :136-138 dynamic_decode, i.e. per step
@@ -224,6 +232,9 @@ int taco_conv_dw(float* dW, int64_t ldw, int64_t tap_stride, const float* X, int
 /* out[n] += sum_m A[m][n] * (Bm ? Bm[m][n] - (R ? R[m][n] : 0) : 1)     (bias / batch-norm gradients) */
 int taco_colsum(float* out, const float* A, int64_t lda, const float* Bm, int64_t ldb, const float* R, int64_t ldr,
                 int M, int N, void* stream);
+/* out[m/period][n] += sum over the `period` rows m of segment m/period of A[m][n]  (per-utterance column sums, e.g. the
+ * gradient of a per-utterance bias); deterministic, no atomics.  M % period == 0.                               */
+int taco_colsum_seg(float* out, int64_t ldo, const float* A, int64_t lda, int M, int N, int period, void* stream);
 /* in place C = act(C + bias) (bias may be NULL); out = X * H[row+shift] (zero outside the period block) */
 int taco_bias_act(float* C, int64_t ldc, int M, int N, const float* bias, int act, void* stream);
 int taco_mul_shift(float* out, int64_t ldo, const float* X, int64_t ldx, const float* H, int64_t ldh, int M, int N,
@@ -255,6 +266,11 @@ int taco_scatter_add_rows(float* dTable, const int32_t* ids, const float* dRows,
 /* serial part of the bidirectional-GRU backward (ops.py:118-128): see csrc/gru_bwd.cu */
 int taco_bigru_bwd(float* dxp, const float* dOut, const float* out, const float* ACT, const float* Wg_h_fw,
                    const float* Wc_h_fw, const float* Wg_h_bw, const float* Wc_h_bw, int B, int T, void* stream);
+/* same, for a forward that started from h0_fw / h0_bw [B][128] (NULL = zero state); dh0 [B][2][128] (or NULL)
+ * receives d(loss)/d(initial state) per direction */
+int taco_bigru_bwd_h0(float* dxp, const float* dOut, const float* out, const float* ACT, const float* Wg_h_fw,
+                      const float* Wc_h_fw, const float* Wg_h_bw, const float* Wc_h_bw, const float* h0_fw,
+                      const float* h0_bw, float* dh0, int B, int T, void* stream);
 /* decoder step inputs of the Training / ScheduledOutputTraining helpers, time-major: Xin [T][B][80], sel [T][B] */
 int taco_dec_inputs(float* Xin, uint8_t* sel, const float* mel, const float* y, const uint8_t* sample_mask, int B, int T,
                     int r, int sched, void* stream);

@@ -32,6 +32,7 @@ class LinearDesc(C.Structure):
         ("epilogue", C.c_int32),
         ("hx", C.c_void_p), ("ldhx", C.c_int64),
         ("pool", C.c_int32), ("impl", C.c_int32),
+        ("bias_utt", C.c_void_p), ("ldbu", C.c_int64),
     ]
 
 
@@ -92,12 +93,12 @@ _lib = None
 # every symbol include/taco_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "taco_last_error", "taco_version", "taco_device_info", "taco_linear_fwd", "taco_pack_weight", "taco_pack_weight_x3",
-    "taco_maxpool_fwd", "taco_gather_rows", "taco_mask_rows", "taco_bigru_fwd",
+    "taco_maxpool_fwd", "taco_gather_rows", "taco_mask_rows", "taco_bigru_fwd", "taco_bigru_fwd_h0",
     "taco_decoder_packed_bytes", "taco_decoder_workspace_bytes", "taco_decoder_pack", "taco_decoder_fwd",
     "taco_l1_loss_fwd", "taco_l1_partial_count", "taco_launch_count",
     # training path
-    "taco_gemm", "taco_set_gemm_impl", "taco_conv_dw", "taco_colsum", "taco_bias_act", "taco_mul_shift", "taco_epi_bwd", "taco_epi_fwd_keep", "taco_bn_param_grad",
-    "taco_maxpool_bwd", "taco_highway_fwd", "taco_highway_bwd", "taco_l1_bwd", "taco_l1_bwd_ld", "taco_scatter_add_rows", "taco_bigru_bwd",
+    "taco_gemm", "taco_set_gemm_impl", "taco_conv_dw", "taco_colsum", "taco_colsum_seg", "taco_bias_act", "taco_mul_shift", "taco_epi_bwd", "taco_epi_fwd_keep", "taco_bn_param_grad",
+    "taco_maxpool_bwd", "taco_highway_fwd", "taco_highway_bwd", "taco_l1_bwd", "taco_l1_bwd_ld", "taco_scatter_add_rows", "taco_bigru_bwd", "taco_bigru_bwd_h0",
     "taco_dec_inputs", "taco_decoder_bwd_workspace_bytes", "taco_decoder_bwd", "taco_attn_bwd_post", "taco_sumsq",
     "taco_adam_step",
     # spectrogram inversion (Griffin-Lim glue kernels)
@@ -129,6 +130,7 @@ def lib():
                                    C.c_void_p, C.c_void_p]
     L.taco_mask_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     L.taco_bigru_fwd.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p]
+    L.taco_bigru_fwd_h0.argtypes = [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_void_p]
     L.taco_decoder_packed_bytes.argtypes = [C.c_int]
     L.taco_decoder_packed_bytes.restype = C.c_size_t
     L.taco_decoder_workspace_bytes.argtypes = [C.c_int] * 4
@@ -141,6 +143,7 @@ def lib():
     vp, i64, i32, f32 = C.c_void_p, C.c_int64, C.c_int, C.c_float
     L.taco_gemm.argtypes = [C.POINTER(GemmDesc), vp]
     L.taco_colsum.argtypes = [vp, vp, i64, vp, i64, vp, i64, i32, i32, vp]
+    L.taco_colsum_seg.argtypes = [vp, i64, vp, i64, i32, i32, i32, vp]
     L.taco_bias_act.argtypes = [vp, i64, i32, i32, vp, i32, vp]
     L.taco_mul_shift.argtypes = [vp, i64, vp, i64, vp, i64, i32, i32, i32, i32, vp]
     L.taco_epi_bwd.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, i32, vp, vp, f32, vp]
@@ -153,6 +156,7 @@ def lib():
     L.taco_l1_bwd_ld.argtypes = [vp, i64, vp, vp, i64, i64, f32, vp]
     L.taco_scatter_add_rows.argtypes = [vp, vp, vp, i32, i32, i32, vp]
     L.taco_bigru_bwd.argtypes = [vp] * 8 + [i32, i32, vp]
+    L.taco_bigru_bwd_h0.argtypes = [vp] * 11 + [i32, i32, vp]
     L.taco_dec_inputs.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     L.taco_decoder_bwd_workspace_bytes.restype = C.c_size_t
     L.taco_decoder_bwd.argtypes = [C.POINTER(DecoderBwdArgs), vp]

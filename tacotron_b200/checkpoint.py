@@ -76,14 +76,23 @@ def restore(model, filename):
     return None, None
 
 
+def num_speakers(filename):
+    """speaker count of a checkpoint written by `save` (rows of its speaker table; 1 for a single-speaker model)"""
+    z = np.load(filename)
+    return int(z["speaker/embed"].shape[0]) if "speaker/embed" in z.files else 1
+
+
 def import_tf_variables(model, tf_vars):
     """{TF-1.2 variable name: ndarray} -> parameter store.  Non-model variables (global_step, Adam slots, stft_mean/std,
-    beta1_power ...) are returned in a dict instead of being loaded."""
+    beta1_power ...) are returned in a dict instead of being loaded.  A bundle with a speaker table
+    (``speaker/speaker_embed``) is read with the multi-speaker name map."""
     params, extra = {}, {}
+    strip = lambda n: n[:-2] if n.endswith(":0") else n
+    multi = any(strip(n) == "speaker/speaker_embed" for n in tf_vars)
     for name, arr in tf_vars.items():
-        name = name[:-2] if name.endswith(":0") else name
+        name = strip(name)
         try:
-            params[tf_name_to_param(name)] = torch.from_numpy(np.asarray(arr, dtype=np.float32))
+            params[tf_name_to_param(name, multi_speaker=multi)] = torch.from_numpy(np.asarray(arr, dtype=np.float32))
         except KeyError:
             extra[name] = arr
     model.load_params(params)

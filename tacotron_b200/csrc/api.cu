@@ -130,6 +130,8 @@ int taco_linear_fwd(const taco_linear_desc* d, void* stream) {
     TACO_CHECK(d->B >= 0 && d->T >= 0 && d->C > 0 && d->N > 0, "taco_linear_fwd: bad sizes B=%d T=%d C=%d N=%d", d->B, d->T, d->C, d->N);
     TACO_CHECK(d->bank_K > 0 || d->taps >= 1, "taco_linear_fwd: taps must be >= 1");
     TACO_CHECK(d->ldx >= d->C, "taco_linear_fwd: ldx < C");
+    TACO_CHECK(!d->bias_utt || (d->epilogue != TACO_EPI_HIGHWAY && d->ldbu >= d->N),
+               "taco_linear_fwd: bias_utt needs the normal epilogue and ldbu >= N");
     if (d->impl == TACO_IMPL_SIMT) return taco_linear_simt(d, (cudaStream_t)stream);
     if (d->impl == TACO_IMPL_TC || d->impl == TACO_IMPL_TC3) return taco_linear_tc(d, (cudaStream_t)stream);
     taco_set_error("taco_linear_fwd: unknown impl %d", d->impl);

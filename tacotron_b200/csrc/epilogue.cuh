@@ -20,10 +20,18 @@ struct EpiParams {
     float          keep_scale;
     int            act;
     int            N;       // valid output columns (for keep-mask row stride and bounds)
+    const float*   bias_utt; // [B][ldbu] per-utterance bias or NULL (row / T = utterance)
+    int64_t        ldbu;
+    int            T;
 };
 
 __device__ __forceinline__ float epi_value(const EpiParams& e, int64_t row, int col, float v) {
-    if (e.bias) v += __ldg(e.bias + col);
+    if (e.bias_utt) {
+        const float bu = __ldg(e.bias_utt + (row / e.T) * e.ldbu + col);
+        v += e.bias ? __ldg(e.bias + col) + bu : bu;
+    } else if (e.bias) {
+        v += __ldg(e.bias + col);
+    }
     v = apply_act(v, e.act);
     if (e.scale) v = v * __ldg(e.scale + col);
     if (e.shift) v = v + __ldg(e.shift + col);

@@ -122,6 +122,7 @@ int taco_linear_simt(const taco_linear_desc* d, cudaStream_t st) {
     a.e.Y = d->Y; a.e.ldy = d->ldy; a.e.bias = d->bias; a.e.scale = d->scale; a.e.shift = d->shift;
     a.e.keep = d->keep; a.e.keep_scale = d->keep_scale; a.e.residual = d->residual; a.e.ldr = d->ldr;
     a.e.hx = d->hx; a.e.ldhx = d->ldhx; a.e.act = d->act; a.e.N = d->N;
+    a.e.bias_utt = d->bias_utt; a.e.ldbu = d->ldbu; a.e.T = d->T;
     const int64_t M = (int64_t)d->B * d->T;
     if (M == 0 || d->N == 0) return 0;
     if (d->epilogue == TACO_EPI_HIGHWAY) {

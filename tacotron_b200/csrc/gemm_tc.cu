@@ -240,6 +240,7 @@ __global__ void __launch_bounds__(TC_THREADS, MODE == 1 ? 1 : 2) gemm_tc_kernel(
                     const int col = n0 + i;
                     const bool cv = col < a.N;
                     cst[i] = (cv && a.e.bias) ? __ldg(a.e.bias + col) : 0.f;
+                    if (cv && a.e.bias_utt) cst[i] += __ldg(a.e.bias_utt + (int64_t)b * a.e.ldbu + col);   // one utterance per tile
                     cst[256 + i] = (cv && a.e.scale) ? __ldg(a.e.scale + col) : 1.f;
                     cst[512 + i] = (cv && a.e.shift) ? __ldg(a.e.shift + col) : 0.f;
                 }
@@ -374,7 +375,8 @@ __global__ void __launch_bounds__(TC_THREADS, MODE == 1 ? 1 : 2) gemm_tc_kernel(
                 }
             } else {
                 const bool cvalid = col < a.N;
-                const float cb = (cvalid && a.e.bias) ? __ldg(a.e.bias + col) : 0.f;
+                float cb = (cvalid && a.e.bias) ? __ldg(a.e.bias + col) : 0.f;
+                if (cvalid && a.e.bias_utt) cb += __ldg(a.e.bias_utt + (int64_t)b * a.e.ldbu + col);
                 const float csc = (cvalid && a.e.scale) ? __ldg(a.e.scale + col) : 1.f;
                 const float csh = (cvalid && a.e.shift) ? __ldg(a.e.shift + col) : 0.f;
                 const int act = a.e.act;
@@ -809,6 +811,7 @@ int taco_linear_tc(const taco_linear_desc* d, cudaStream_t st) {
     a.e.Y = d->Y; a.e.ldy = d->ldy; a.e.bias = d->bias; a.e.scale = d->scale; a.e.shift = d->shift;
     a.e.keep = d->keep; a.e.keep_scale = d->keep_scale; a.e.residual = d->residual; a.e.ldr = d->ldr;
     a.e.hx = d->hx; a.e.ldhx = d->ldhx; a.e.act = d->act; a.e.N = highway ? d->N / 2 : d->N;
+    a.e.bias_utt = d->bias_utt; a.e.ldbu = d->ldbu; a.e.T = d->T;
 
     const int max_taps = d->bank_K > 0 ? d->bank_K : d->taps;
     TACO_CHECK(d->ldwp >= (int64_t)max_taps * a.Cpad, "taco_linear_fwd(TC): ldwp too small for taps*Cpad");

@@ -31,7 +31,8 @@ __device__ __forceinline__ void ffma2(float2& d, const float2 a, const float2 b)
 
 __global__ void __launch_bounds__(512, 1)
 bigru_kernel(const float* __restrict__ xp, const float* __restrict__ Wg_fw, const float* __restrict__ Wc_fw,
-             const float* __restrict__ Wg_bw, const float* __restrict__ Wc_bw, float* __restrict__ out, int T) {
+             const float* __restrict__ Wg_bw, const float* __restrict__ Wc_bw, const float* __restrict__ h0_fw,
+             const float* __restrict__ h0_bw, float* __restrict__ out, int T) {
     const int b = blockIdx.x;
     const int dir = blockIdx.y;
     const int tid = threadIdx.x, lane = tid & 31;
@@ -70,7 +71,8 @@ bigru_kernel(const float* __restrict__ xp, const float* __restrict__ Wg_fw, cons
     const bool g_owner = (l3 & 1) == 0;
     const bool c_owner = (l3 & 3) == 0;
 
-    if (tid < H) h_s[tid] = 0.0f;               // zero initial state (ops.py:112-115, s is None)
+    const float* h0 = dir ? h0_bw : h0_fw;     // initial state (ops.py:111-126): speaker-dependent, or NULL = zero state
+    if (tid < H) h_s[tid] = h0 ? __ldg(h0 + b * H + tid) : 0.0f;
     __syncthreads();
 
     // pointers advance by one time step per iteration (no per-step index arithmetic); the input products are prefetched
@@ -167,14 +169,20 @@ bigru_kernel(const float* __restrict__ xp, const float* __restrict__ Wg_fw, cons
 
 }  // namespace
 
-extern "C" int taco_bigru_fwd(const float* xp, const float* Wg_h_fw, const float* Wc_h_fw, const float* Wg_h_bw,
-                              const float* Wc_h_bw, float* out, int B, int T, void* stream) {
+extern "C" int taco_bigru_fwd_h0(const float* xp, const float* Wg_h_fw, const float* Wc_h_fw, const float* Wg_h_bw,
+                                 const float* Wc_h_bw, const float* h0_fw, const float* h0_bw, float* out, int B, int T,
+                                 void* stream) {
     TACO_CHECK(xp && Wg_h_fw && Wc_h_fw && Wg_h_bw && Wc_h_bw && out, "taco_bigru_fwd: NULL pointer");
     TACO_CHECK(B >= 0 && T >= 0, "taco_bigru_fwd: negative size");
     TACO_CHECK((int64_t)B * T * 768 < (int64_t)1 << 31, "taco_bigru_fwd: B*T = %lld too large for 32-bit offsets", (long long)B * T);
     if (B == 0 || T == 0) return 0;
     dim3 grid(B, 2);
-    bigru_kernel<<<grid, 512, 0, (cudaStream_t)stream>>>(xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, out, T);
+    TACO_LAUNCH(bigru_kernel, grid, 512, 0, (cudaStream_t)stream, xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw, out, T);
     TACO_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int taco_bigru_fwd(const float* xp, const float* Wg_h_fw, const float* Wc_h_fw, const float* Wg_h_bw,
+                              const float* Wc_h_bw, float* out, int B, int T, void* stream) {
+    return taco_bigru_fwd_h0(xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, nullptr, nullptr, out, B, T, stream);
 }

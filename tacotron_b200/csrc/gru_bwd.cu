@@ -45,12 +45,14 @@ __device__ __forceinline__ float butterfly8(float (&p)[8], int lane) {
 __global__ void __launch_bounds__(512, 1)
 bigru_bwd_kernel(float* __restrict__ dxp, const float* __restrict__ dOut, const float* __restrict__ out, const float* __restrict__ ACT,
                  const float* __restrict__ Wg_fw, const float* __restrict__ Wc_fw, const float* __restrict__ Wg_bw,
-                 const float* __restrict__ Wc_bw, int T) {
+                 const float* __restrict__ Wc_bw, const float* __restrict__ h0_fw, const float* __restrict__ h0_bw,
+                 float* __restrict__ dh0, int T) {
     const int b = blockIdx.x;
     const int dir = blockIdx.y;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const float* Wg = dir ? Wg_bw : Wg_fw;     // [128][256]  h-side rows of the gates kernel
     const float* Wc = dir ? Wc_bw : Wc_fw;     // [128][128]  (r*h)-side rows of the candidate kernel
+    const float* h0 = dir ? h0_bw : h0_fw;     // initial state [B][128] or NULL (zero): hprev of the first processed step
 
     __shared__ __align__(16) float dc_s[H];        // dc_pre
     __shared__ __align__(16) float dg_s[2 * H];    // [dr_pre | du_pre]
@@ -81,7 +83,7 @@ bigru_bwd_kernel(float* __restrict__ dxp, const float* __restrict__ dOut, const 
             const int n = tid;
             const float* a = ACT + (seq + t) * 768 + dir * 384;
             const float r = a[n], u = a[H + n], c = a[2 * H + n];
-            const float hprev = (tp >= 0 && tp < T) ? out[(seq + tp) * 256 + dir * H + n] : 0.f;
+            const float hprev = (tp >= 0 && tp < T) ? out[(seq + tp) * 256 + dir * H + n] : (h0 ? h0[b * H + n] : 0.f);
             const float dh = dOut[(seq + t) * 256 + dir * H + n] + carry_s[n];
             const float du_pre = dh * (hprev - c) * u * (1.0f - u);
             const float dc_pre = dh * (1.0f - u) * (1.0f - c * c);
@@ -134,16 +136,24 @@ bigru_bwd_kernel(float* __restrict__ dxp, const float* __restrict__ dOut, const 
         }
         __syncthreads();
     }
+    if (dh0 && tid < H) dh0[(b * 2 + dir) * H + tid] = carry_s[tid];     // d(loss)/d(initial state)
 }
 
 }  // namespace
 
-extern "C" int taco_bigru_bwd(float* dxp, const float* dOut, const float* out, const float* ACT, const float* Wg_h_fw,
-                              const float* Wc_h_fw, const float* Wg_h_bw, const float* Wc_h_bw, int B, int T, void* stream) {
+extern "C" int taco_bigru_bwd_h0(float* dxp, const float* dOut, const float* out, const float* ACT, const float* Wg_h_fw,
+                                 const float* Wc_h_fw, const float* Wg_h_bw, const float* Wc_h_bw, const float* h0_fw,
+                                 const float* h0_bw, float* dh0, int B, int T, void* stream) {
     TACO_CHECK(dxp && dOut && out && ACT && Wg_h_fw && Wc_h_fw && Wg_h_bw && Wc_h_bw, "taco_bigru_bwd: NULL pointer");
     TACO_CHECK(B >= 0 && T >= 0, "taco_bigru_bwd: negative size");
-    if (B == 0 || T == 0) return 0;
-    TACO_LAUNCH(bigru_bwd_kernel, dim3(B, 2), 512, 0, (cudaStream_t)stream, dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, T);
+    if (B == 0 || (T == 0 && !dh0)) return 0;             // T == 0 with dh0: the kernel only writes dh0 = 0
+    TACO_LAUNCH(bigru_bwd_kernel, dim3(B, 2), 512, 0, (cudaStream_t)stream, dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw,
+                h0_fw, h0_bw, dh0, T);
     TACO_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int taco_bigru_bwd(float* dxp, const float* dOut, const float* out, const float* ACT, const float* Wg_h_fw,
+                              const float* Wc_h_fw, const float* Wg_h_bw, const float* Wc_h_bw, int B, int T, void* stream) {
+    return taco_bigru_bwd_h0(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, nullptr, nullptr, nullptr, B, T, stream);
 }

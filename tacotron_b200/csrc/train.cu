@@ -528,6 +528,27 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     }
 }
 
+// per-segment column sums: block (column chunk, segment) reduces the `period` rows of its segment in a fixed order and is the
+// only writer of its 32 outputs -- deterministic without atomics
+__global__ void __launch_bounds__(256) colsum_seg_kernel(float* __restrict__ out, int64_t ldo, const float* __restrict__ A,
+                                                         int64_t lda, int N, int period) {
+    __shared__ float red[8][33];
+    const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
+    const int n = blockIdx.x * 32 + x;
+    const int64_t r0 = (int64_t)blockIdx.y * period;
+    float acc = 0.f;
+    if (n < N)
+        for (int m = y; m < period; m += 8) acc += A[(r0 + m) * lda + n];
+    red[y][x] = acc;
+    __syncthreads();
+    if (y == 0 && n < N) {
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) s += red[w][x];
+        out[(int64_t)blockIdx.y * ldo + n] += s;
+    }
+}
+
 }  // namespace
 
 static int g_gemm_impl = 0;        // taco_set_gemm_impl
@@ -575,6 +596,15 @@ int taco_set_gemm_impl(int impl) {
     const int prev = g_gemm_impl;
     if (impl == 0 || impl == 1) g_gemm_impl = impl;
     return prev;
+}
+
+int taco_colsum_seg(float* out, int64_t ldo, const float* A, int64_t lda, int M, int N, int period, void* stream) {
+    TACO_CHECK(out && A && M >= 0 && N >= 0 && period >= 1 && M % period == 0 && ldo >= N,
+               "taco_colsum_seg: bad arguments (M=%d N=%d period=%d)", M, N, period);
+    if (M == 0 || N == 0) return 0;
+    TACO_LAUNCH(colsum_seg_kernel, dim3((N + 31) / 32, M / period), 256, 0, (cudaStream_t)stream, out, ldo, A, lda, N, period);
+    TACO_LAUNCH_CHECK();
+    return 0;
 }
 
 #ifndef TACO_HOST_EMU   /* the remaining entry points launch with <<<>>> directly (not part of the host emulation) */

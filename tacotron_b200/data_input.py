@@ -82,7 +82,7 @@ def shuffled_indices(n, buffer_size=SHUFFLE_BUFFER_SIZE, seed=0):
 
 class DeviceBatches:
     """``build_dataset`` (data_input.py:20-40) for a CUDA consumer: iterator of input dicts of DEVICE tensors
-    {'text' i32 [B,Tx], 'text_length' i32 [B], 'stft' f32 [B,T,1025r], 'mel' f32 [B,T,80r], 'speech_length' i32 [B]}.
+    {'text' i32 [B,Tx], 'text_length' i32 [B], 'stft' f32 [B,T,1025r], 'mel' f32 [B,T,80r], 'speech_length' i32 [B]}, plus 'speaker' i32 [B] when the arrays have speaker ids.
     shard=(rank, world): data parallel ranks draw disjoint batches from the same shuffled stream."""
 
     def __init__(self, arrays, batch_size=BATCH_SIZE, buffer_size=SHUFFLE_BUFFER_SIZE, seed=0, device="cuda", shard=(0, 1), K=None):
@@ -114,6 +114,8 @@ class DeviceBatches:
         h = {"text": host((B,) + a["text"].shape[1:], torch.int32), "text_length": host((B,), torch.int32),
              "speech_length": host((B,), torch.int32), "stft": host((B,) + a["stft"].shape[1:], torch.float16),
              "mel": host((B,) + a["mel"].shape[1:], torch.float16)}
+        if "speaker" in a:                            # multi-speaker corpus (speakers.npy, data_input.py:79-83)
+            h["speaker"] = host((B,), torch.int32)
         d = {k: torch.empty(v.shape, dtype=v.dtype, device=self.device) for k, v in h.items()}
         out = {"stft": torch.empty(h["stft"].shape, dtype=torch.float32, device=self.device),
                "mel": torch.empty(h["mel"].shape, dtype=torch.float32, device=self.device)}
@@ -133,7 +135,7 @@ class DeviceBatches:
             if s["used"]:
                 s["ready"].synchronize()              # the previous H2D out of these pinned buffers has completed
         ids = self._next_indices()
-        for k in ("text", "text_length", "speech_length", "stft", "mel"):
+        for k in s["h"]:
             s["h"][k].copy_(torch.from_numpy(np.ascontiguousarray(self.a[k][ids])))
         ctx = torch.cuda.stream(self.stream) if self.cuda else _null()
         with ctx:
@@ -164,8 +166,11 @@ class DeviceBatches:
         if self.cuda and self.slots[self.cur]["used"]:
             self.slots[self.cur]["free"].record()    # everything that reads the previous batch is already enqueued
         self._launch(self.cur)                       # stage the following batch while this one is consumed
-        return {"text": s["d"]["text"], "text_length": s["d"]["text_length"], "speech_length": s["d"]["speech_length"],
-                "stft": s["out"]["stft"], "mel": s["out"]["mel"]}
+        batch = {"text": s["d"]["text"], "text_length": s["d"]["text_length"], "speech_length": s["d"]["speech_length"],
+                 "stft": s["out"]["stft"], "mel": s["out"]["mel"]}
+        if "speaker" in s["d"]:
+            batch["speaker"] = s["d"]["speaker"]
+        return batch
 
 
 class _null:

@@ -278,6 +278,34 @@ def bigru_bwd(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw):
                                    _st()), "taco_bigru_bwd")
 
 
+def bigru_bwd_h0(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw, dh0):
+    B, T, _ = out.shape
+    for t in (dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw, dh0):
+        assert t is None or (t.is_contiguous() and t.is_cuda)
+    for t in (h0_fw, h0_bw):
+        assert t is None or tuple(t.shape) == (B, 128)
+    assert dh0 is None or tuple(dh0.shape) == (B, 2, 128)
+    L.check(L.lib().taco_bigru_bwd_h0(_p(dxp), _p(dOut), _p(out), _p(ACT), _p(Wg_h_fw), _p(Wc_h_fw), _p(Wg_h_bw), _p(Wc_h_bw),
+                                      _p(h0_fw), _p(h0_bw), _p(dh0), B, T, _st()), "taco_bigru_bwd_h0")
+
+
+def bigru_fwd_h0(out, xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw):
+    B, T, _ = out.shape
+    for t in (out, xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw):
+        assert t is None or (t.is_contiguous() and t.is_cuda)
+    for t in (h0_fw, h0_bw):
+        assert t is None or tuple(t.shape) == (B, 128)
+    L.check(L.lib().taco_bigru_fwd_h0(_p(xp), _p(Wg_h_fw), _p(Wc_h_fw), _p(Wg_h_bw), _p(Wc_h_bw), _p(h0_fw), _p(h0_bw), _p(out),
+                                      B, T, _st()), "taco_bigru_fwd_h0")
+
+
+def colsum_seg(out, A, period):
+    _chk2(A, "colsum_seg A"); _chk2(out, "colsum_seg out")
+    M, N = A.shape
+    assert M % period == 0 and tuple(out.shape) == (M // period, N), (out.shape, A.shape, period)
+    L.check(L.lib().taco_colsum_seg(_p(out), _ld(out), _p(A), _ld(A), M, N, period, _st()), "taco_colsum_seg")
+
+
 def dec_inputs(Xin, sel, mel, y, sample_mask, r, sched):
     T, B, mf = Xin.shape
     assert mf == 80 and sel.dtype == torch.uint8 and mel.is_contiguous() and y.is_contiguous()

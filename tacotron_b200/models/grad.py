@@ -85,9 +85,11 @@ def S_affine(P, pre):
 # ------------------------------------------------------------------------------------------------------------
 # highway (models/ops.py:27-46)
 # ------------------------------------------------------------------------------------------------------------
-def highway_bwd(K, P, G, S, pre, tag, dY, x_outer=None):
+def highway_bwd(K, P, G, S, pre, tag, dY, x_outer=None, spk=None):
     """dY [M,128] -> gradient w.r.t. the layer input.  S[tag+'_in'] = input of the T/H denses (after the optional
-    width-changing dense), S[tag+'_P'] = [h_pre | t_pre].  x_outer = input of the optional dense (ops.py:29-30)."""
+    width-changing dense), S[tag+'_P'] = [h_pre | t_pre].  x_outer = input of the optional dense (ops.py:29-30).
+    spk = (s_l [B,128], ds_l [B,128], T) for a speaker-conditioned layer (ops.py:101-107): its dense sees [x_outer | s_l],
+    computed forward as x_outer.Wd[:128] + u, u = s_l.Wd[128:] + bd per utterance; ds_l is accumulated into."""
     X = _v2(S[f"{tag}_in"])
     Pm = _v2(S[f"{tag}_P"])
     M, U = X.shape
@@ -101,6 +103,18 @@ def highway_bwd(K, P, G, S, pre, tag, dY, x_outer=None):
     K.gemm(G[f"{pre}/WT"], X, dT, ta=True, beta=1.0)
     K.colsum(G[f"{pre}/bH"], dH)
     K.colsum(G[f"{pre}/bT"], dT)
+    if spk is not None:
+        s_l, ds_l, T = spk
+        Wd = P[f"{pre}/Wd"]
+        Xo = _v2(x_outer)
+        dXo = K.empty(Xo.shape, dY)
+        dense_bwd(K, dX, Xo, Wd[:128], G[f"{pre}/Wd"][:128], dX=dXo)
+        du = K.zeros((Xo.shape[0] // T, U), dY)
+        K.colsum_seg(du, dX, T)                                  # du[b] = sum_t d(proj)[b,t]
+        K.gemm(G[f"{pre}/Wd"][128:], s_l, du, ta=True, beta=1.0)
+        K.colsum(G[f"{pre}/bd"], du)
+        K.gemm(ds_l, du, Wd[128:], tb=True, beta=1.0)
+        return dXo
     if f"{pre}/Wd" in P:
         Xo = _v2(x_outer)
         dXo = K.empty(Xo.shape, dY)
@@ -112,31 +126,43 @@ def highway_bwd(K, P, G, S, pre, tag, dY, x_outer=None):
 # ------------------------------------------------------------------------------------------------------------
 # bidirectional GRU (models/ops.py:118-128, SURVEY A.5)
 # ------------------------------------------------------------------------------------------------------------
-def bigru_bwd(K, P, G, S, p, dOut):
-    """dOut [B,T,256] -> dHin [B*T,128]."""
+def bigru_bwd(K, P, G, S, p, dOut, dh0=None):
+    """dOut [B,T,256] -> dHin [B*T,128].  When the forward started from an initial state S[p+'/h0'] [B,128] (both
+    directions, ops.py:111-126), dh0 [B,2,128] receives d(loss)/d(initial state) per direction."""
     out, xp, hin = S[f"{p}/gru_out"], S[f"{p}/xp"], S[f"{p}/hw_out"]
+    h0 = S.get(f"{p}/h0")
     B, T, _ = out.shape
     M = B * T
     out2, hin2 = _v2(out), _v2(hin)
     ACT = K.empty((M, 768), out)
     ACT.copy_(_v2(xp))                                   # x-side products + biases (data movement only)
     RH = K.empty((M, 256), out)
+    ACT3, RH3 = ACT.view(B, T, 768), RH.view(B, T, 256)
     names = (f"{p}/gru_fw", f"{p}/gru_bw")
     for d, dn in enumerate(names):
         Wg, Wc = P[f"{dn}/Wg"], P[f"{dn}/Wc"]
         sh = -1 if d == 0 else 1                         # h(t-1) in processing order: previous row (fw) / next row (bw)
+        first = 0 if d == 0 else T - 1                   # first processed step: its h(t-1) is the initial state
         Hd = out2[:, d * 128:(d + 1) * 128]
         g = ACT[:, d * 384:d * 384 + 256]
         c = ACT[:, d * 384 + 256:(d + 1) * 384]
         K.gemm(g, Hd, Wg[128:], beta=1.0, shift=sh, period=T)
+        if h0 is not None:
+            K.gemm(ACT3[:, first, d * 384:d * 384 + 256], h0, Wg[128:], beta=1.0)
         K.bias_act_(g, None, ACT_SIGMOID)
         RHd = RH[:, d * 128:(d + 1) * 128]
         K.mul_shift(RHd, g[:, :128], Hd, sh, T)
+        if h0 is not None:
+            K.mul_shift(RH3[:, first, d * 128:(d + 1) * 128], ACT3[:, first, d * 384:d * 384 + 128], h0, 0, 0)
         K.gemm(c, RHd, Wc[128:], beta=1.0)
         K.bias_act_(c, None, ACT_TANH)
     dxp = K.empty((M, 768), out)
-    K.bigru_bwd(dxp.view(B, T, 768), dOut, out, ACT.view(B, T, 768), P[f"{names[0]}/Wg"][128:], P[f"{names[0]}/Wc"][128:],
-                P[f"{names[1]}/Wg"][128:], P[f"{names[1]}/Wc"][128:])
+    if h0 is None:
+        K.bigru_bwd(dxp.view(B, T, 768), dOut, out, ACT.view(B, T, 768), P[f"{names[0]}/Wg"][128:], P[f"{names[0]}/Wc"][128:],
+                    P[f"{names[1]}/Wg"][128:], P[f"{names[1]}/Wc"][128:])
+    else:
+        K.bigru_bwd_h0(dxp.view(B, T, 768), dOut, out, ACT.view(B, T, 768), P[f"{names[0]}/Wg"][128:], P[f"{names[0]}/Wc"][128:],
+                       P[f"{names[1]}/Wg"][128:], P[f"{names[1]}/Wc"][128:], h0, h0, dh0)
     if "_capture" in S:
         S["_capture"][f"{p}/bigru_bwd"] = {"dxp": dxp.view(B, T, 768), "dOut": dOut, "out": out, "ACT": ACT.view(B, T, 768)}
     dHin = K.empty((M, 128), out)
@@ -151,6 +177,9 @@ def bigru_bwd(K, P, G, S, p, dOut):
         K.gemm(dHin, dc, Wc[:128], tb=True, beta=1.0)
         K.gemm(G[f"{dn}/Wg"][:128], hin2, dg, ta=True, beta=1.0)
         K.gemm(G[f"{dn}/Wg"][128:], Hd, dg, ta=True, beta=1.0, shift=sh, period=T)
+        if h0 is not None:
+            first = 0 if d == 0 else T - 1
+            K.gemm(G[f"{dn}/Wg"][128:], h0, dxp.view(B, T, 768)[:, first, d * 384:d * 384 + 256], ta=True, beta=1.0)
         K.gemm(G[f"{dn}/Wc"][:128], hin2, dc, ta=True, beta=1.0)
         K.gemm(G[f"{dn}/Wc"][128:], RHd, dc, ta=True, beta=1.0)
         K.colsum(G[f"{dn}/bg"], dg)
@@ -167,9 +196,18 @@ def cbhg_bwd(K, P, G, S, p, dOut, Kb, c, n_hw=4):
     B, T, Cin = x_in.shape
     X = _v2(x_in)
     M = B * T
-    dH = bigru_bwd(K, P, G, S, p, dOut)                                       # [M,128]
+    Sv = S.get(f"{p}/spk_s")                                                  # speaker-conditioned CBHG (ops.py:101-115)
+    dh0 = K.empty((B, 2, 128), dOut) if Sv is not None else None
+    dH = bigru_bwd(K, P, G, S, p, dOut, dh0=dh0)                              # [M,128]
+    dSv = K.zeros(Sv.shape, dOut) if Sv is not None else None
     for l in range(n_hw - 1, -1, -1):
-        dH = highway_bwd(K, P, G, S, f"{p}/highway{l}", f"{p}/hw{l}", dH, x_outer=S[f"{p}/res"])
+        if Sv is not None:
+            spk = (Sv[:, 128 * l:128 * (l + 1)], dSv[:, 128 * l:128 * (l + 1)], T)
+            dH = highway_bwd(K, P, G, S, f"{p}/highway{l}", f"{p}/hw{l}", dH, x_outer=S[f"{p}/hw{l}_x"], spk=spk)
+        else:
+            dH = highway_bwd(K, P, G, S, f"{p}/highway{l}", f"{p}/hw{l}", dH, x_outer=S[f"{p}/res"])
+    if Sv is not None:
+        speaker_bwd(K, P, G, S, p, dSv, dh0, n_hw)
     dRes = dH                                                                  # [M,Cin]  (res = proj2_bn + x_in)
     dIn = K.empty((M, Cin), dRes)
     dIn.copy_(dRes)                                                            # residual branch (ops.py:92)
@@ -193,6 +231,23 @@ def cbhg_bwd(K, P, G, S, p, dOut, Kb, c, n_hw=4):
         conv_bwd(K, dBank[:, (k - 1) * co:k * co], X, P[f"{p}/bank/W{k}"], G[f"{p}/bank/W{k}"], G[f"{p}/bank/b{k}"], T,
                  dX=dIn, beta_dx=1.0)
     return dIn
+
+
+def speaker_bwd(K, P, G, S, p, dSv, dh0, n_hw):
+    """Reverse of ops._speaker_terms: S = relu(e.[Ws_0 .. Ws_{n-1} | Ws_init] + bs), e = speaker table rows of
+    S['speaker'].  dSv [B,128*(n_hw+1)] holds the highway layers' ds_l; the initial-state block gets dh0_fw + dh0_bw."""
+    Sv, e = S[f"{p}/spk_s"], S[f"{p}/spk_e"]
+    B = Sv.shape[0]
+    K.colsum_seg(dSv[:, 128 * n_hw:], dh0.view(2 * B, 128), 2)                # both directions start from the same state
+    K.epi_bwd(dSv, dSv, Sv, True)                                              # relu
+    de = K.empty(e.shape, e)
+    names = [f"highway{l}" for l in range(n_hw)] + ["gru_init"]
+    for i, nm in enumerate(names):
+        blk = dSv[:, 128 * i:128 * (i + 1)]
+        K.gemm(G[f"{p}/{nm}/Ws"], e, blk, ta=True, beta=1.0)
+        K.colsum(G[f"{p}/{nm}/bs"], blk)
+        K.gemm(de, blk, P[f"{p}/{nm}/Ws"], tb=True, beta=0.0 if i == 0 else 1.0)
+    K.scatter_add_rows(G["speaker/embed"], S["speaker"], de)
 
 
 # ------------------------------------------------------------------------------------------------------------

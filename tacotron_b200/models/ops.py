@@ -167,7 +167,7 @@ def bn_affine(rt, sc):
 # the one contraction primitive
 # ----------------------------------------------------------------------------------------------
 def linear(rt, x, W, Wp, N, *, taps=1, bank_K=0, bank_cout=0, bias=None, act=L.ACT_NONE, scale=None, shift=None,
-           keep=None, keep_scale=1.0, residual=None, highway_x=None, pool=False, out=None, tag="lin"):
+           keep=None, keep_scale=1.0, residual=None, highway_x=None, pool=False, out=None, tag="lin", bias_utt=None):
     """x [B,T,C] (contiguous) -> [B,T,N'] through taco_linear_fwd.  See include/taco_b200.h."""
     assert x.dim() == 3 and x.is_cuda and x.dtype == torch.float32 and x.stride(2) == 1
     B, T, Cin = x.shape
@@ -198,6 +198,9 @@ def linear(rt, x, W, Wp, N, *, taps=1, bank_K=0, bank_cout=0, bias=None, act=L.A
         d.epilogue = L.EPI_HIGHWAY
         d.hx = highway_x.data_ptr(); d.ldhx = highway_x.stride(-2)
     d.pool = 1 if pool else 0
+    if bias_utt is not None:                                    # [B, >= N] per-utterance bias, unit inner stride
+        assert bias_utt.dim() == 2 and bias_utt.shape[0] == B and bias_utt.stride(1) == 1
+        d.bias_utt = bias_utt.data_ptr(); d.ldbu = bias_utt.stride(0)
     d.impl = rt.impl
     L.check(L.lib().taco_linear_fwd(C.byref(d), L.current_stream()), f"taco_linear_fwd[{tag}]")
     return out
@@ -320,7 +323,9 @@ highwaynet = highway
 # ----------------------------------------------------------------------------------------------
 # bidirectional GRU (models/ops.py:118-128)
 # ----------------------------------------------------------------------------------------------
-def bidirectional_gru(inputs, gru_units=128, scope=None):
+def bidirectional_gru(inputs, gru_units=128, scope=None, h0=None):
+    """h0: None (zero state) or the [B,128] initial state of both directions (initial_state_fw = initial_state_bw,
+    models/ops.py:111-126)"""
     sc = scope or current_scope()
     rt = runtime(sc.store)
     assert gru_units == 128 and inputs.shape[-1] == 128, "the persistent GRU kernel is specialised for 128 units"
@@ -342,8 +347,14 @@ def bidirectional_gru(inputs, gru_units=128, scope=None):
     bx = rt.get(("gru_bx", sc.prefix), build_b)
     xp = linear(rt, inputs, Wx, packed_weight(rt, sc.name("gru_wx"), Wx, 1, Cin, 768), 768, bias=bx, tag=sc.name("xp"))
     out = rt.buf(sc.name("gru_out"), (B, T, 2 * gru_units))
-    L.check(L.lib().taco_bigru_fwd(L.ptr(xp), L.ptr(fw.p("Wg")[Cin:]), L.ptr(fw.p("Wc")[Cin:]), L.ptr(bw.p("Wg")[Cin:]),
-                                   L.ptr(bw.p("Wc")[Cin:]), L.ptr(out), B, T, L.current_stream()), "taco_bigru_fwd")
+    if h0 is None:
+        L.check(L.lib().taco_bigru_fwd(L.ptr(xp), L.ptr(fw.p("Wg")[Cin:]), L.ptr(fw.p("Wc")[Cin:]), L.ptr(bw.p("Wg")[Cin:]),
+                                       L.ptr(bw.p("Wc")[Cin:]), L.ptr(out), B, T, L.current_stream()), "taco_bigru_fwd")
+    else:
+        assert h0.shape == (B, gru_units) and h0.is_contiguous()
+        L.check(L.lib().taco_bigru_fwd_h0(L.ptr(xp), L.ptr(fw.p("Wg")[Cin:]), L.ptr(fw.p("Wc")[Cin:]), L.ptr(bw.p("Wg")[Cin:]),
+                                          L.ptr(bw.p("Wc")[Cin:]), L.ptr(h0), L.ptr(h0), L.ptr(out), B, T, L.current_stream()),
+                "taco_bigru_fwd_h0")
     if _save is not None:
         _save[sc.name("hw_out")] = inputs; _save[sc.name("xp")] = xp; _save[sc.name("gru_out")] = out
     return out
@@ -352,10 +363,46 @@ def bidirectional_gru(inputs, gru_units=128, scope=None):
 # ----------------------------------------------------------------------------------------------
 # CBHG (models/ops.py:48-132)
 # ----------------------------------------------------------------------------------------------
+def _speaker_terms(sc, e, n_hw):
+    """Speaker conditioning of a CBHG (models/ops.py:101-115) from e [B,16]: the n_hw highway speaker denses and the
+    bi-GRU initial-state dense as ONE contraction over the concatenated [16, 128*(n_hw+1)] weight (S = relu(e.Ws + bs)),
+    then per highway layer the per-utterance part of its width-fixing dense, u_l = s_l.Wd_l[128:] + bd_l.
+    Returns (S [B,128*(n_hw+1)], [u_l [B,128]], h0 [B,128] contiguous)."""
+    rt = runtime(sc.store)
+    B, E = e.shape
+    names = [f"highway{l}" for l in range(n_hw)] + ["gru_init"]
+
+    def build_w(old):
+        w = torch.cat([sc.p(f"{n}/Ws") for n in names], dim=1)
+        if old is not None:
+            old.copy_(w); return old
+        return w.contiguous()
+
+    def build_b(old):
+        b = torch.cat([sc.p(f"{n}/bs") for n in names])
+        if old is not None:
+            old.copy_(b); return old
+        return b.contiguous()
+    Ws = rt.get(("spk_w", sc.prefix), build_w)
+    bs = rt.get(("spk_b", sc.prefix), build_b)
+    NS = 128 * len(names)
+    Sv = linear(rt, e.view(1, B, E), Ws, packed_weight(rt, sc.name("spk_w"), Ws, 1, E, NS), NS, bias=bs, act=L.ACT_RELU,
+                tag=sc.name("spk_s")).view(B, NS)
+    us = []
+    for l in range(n_hw):
+        Wu = sc.p(f"highway{l}/Wd")[128:]
+        u = linear(rt, Sv.view(1, B, NS)[:, :, 128 * l:128 * (l + 1)], Wu, packed_weight(rt, sc.name(f"highway{l}/Wd_s"), Wu, 1, 128, 128),
+                   128, bias=sc.p(f"highway{l}/bd"), tag=sc.name(f"highway{l}/u"))
+        us.append(u.view(B, 128))
+    h0 = rt.buf(sc.name("gru_h0"), (B, 128))
+    h0.copy_(Sv[:, 128 * n_hw:])                                  # the kernel reads [B][128] rows (data movement only)
+    return Sv, us, h0
+
+
 def CBHG(inputs, speaker_embed=None, K=16, c=[128, 128, 128], gru_units=128, num_highway_layers=4, num_conv_proj=2,
          trace=None):
-    if speaker_embed is not None:
-        raise NotImplementedError("multi-speaker path (ops.py:101-115) is out of scope: num_speakers == 1")
+    """speaker_embed: None, or e [B,16] (multi-speaker encoder, models/ops.py:101-115): layer l's highway input is
+    [h | tile(s_l)], computed as h.Wd_l[:128] plus the per-utterance bias u_l; the bi-GRU starts from relu(e.Wg + bg)."""
     assert num_conv_proj == len(c) - 1                           # ops.py:75
     with variable_scope("cbhg") as sc:
         rt = runtime(sc.store)
@@ -383,14 +430,28 @@ def CBHG(inputs, speaker_embed=None, K=16, c=[128, 128, 128], gru_units=128, num
             _save[sc.name("x_in")] = inputs
             _save[sc.name("bank_bn")] = _save[sc.name("bank/bn")]
             _save[sc.name("bank_pool")] = conv_bank
+        h0 = None
+        if speaker_embed is not None:
+            assert speaker_embed.shape == (B, 16) and speaker_embed.is_contiguous()
+            Sv, us, h0 = _speaker_terms(sc, speaker_embed, num_highway_layers)
+            if _save is not None:
+                _save[sc.name("spk_e")] = speaker_embed; _save[sc.name("spk_s")] = Sv; _save[sc.name("h0")] = h0
         for layer in range(num_highway_layers):
-            h = highway(h, scope=sc.sub(f"highway{layer}"))
+            hsc = sc.sub(f"highway{layer}")
+            if speaker_embed is not None:                         # width-fixing dense of [h | tile(s_l)] (ops.py:29-30)
+                Wx = hsc.p("Wd")[:128]
+                x_outer = h
+                h = linear(rt, h, Wx, packed_weight(rt, hsc.name("Wd_x"), Wx, 1, 128, 128), 128, bias_utt=us[layer],
+                           tag=hsc.name("d"))
+                if _save is not None:
+                    _save[sc.name(f"hw{layer}_x")] = x_outer
+            h = highway(h, scope=hsc)
             if _save is not None:
                 _save[sc.name(f"hw{layer}_in")] = _save[sc.name(f"highway{layer}/in")]
                 _save[sc.name(f"hw{layer}_P")] = _save[sc.name(f"highway{layer}/P")]
         if trace is not None:
             trace[sc.name("highway_out")] = h
-        out = bidirectional_gru(h, gru_units, scope=sc)
+        out = bidirectional_gru(h, gru_units, scope=sc, h0=h0)
         if trace is not None:
             trace[sc.name("out")] = out
         return out

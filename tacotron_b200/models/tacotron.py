@@ -61,8 +61,8 @@ class Tacotron(object):
         """Reference signature ``Tacotron(config, inputs, train)`` (tacotron.py:187).  `inputs` may be
         None (build only) or the input dict of tensors; when given the forward (and loss, if train)
         is evaluated immediately so the result attributes exist as they do after a sess.run."""
-        if config.num_speakers != 1:
-            raise NotImplementedError("multi-speaker (tacotron.py:116-124) is out of scope")
+        if config.num_speakers > 1 and getattr(config, "speaker_embed_dim", 16) != 16:
+            raise ValueError("speaker_embed_dim must be 16 (models/tacotron.py:30)")
         if not torch.cuda.is_available():
             raise RuntimeError("tacotron_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         L.lib()                                   # fail loudly if the extension is missing
@@ -135,13 +135,32 @@ class Tacotron(object):
         return run
 
     # -- inference (tacotron.py:107-154) --------------------------------------------------------
+    def _speaker_embed(self, inputs):
+        """e [B,16] = speaker table rows of inputs['speaker'] (tacotron.py:116-124), or None for a single-speaker model
+        (which ignores a 'speaker' key, as the reference does)"""
+        if self.config.num_speakers <= 1:
+            return None
+        spk = inputs.get("speaker")
+        if spk is None:
+            raise ValueError(f"a model with num_speakers = {self.config.num_speakers} needs inputs['speaker'] (int32 [B])")
+        B = inputs["text"].shape[0]
+        if not (spk.dtype == torch.int32 and spk.is_cuda and spk.is_contiguous() and tuple(spk.shape) == (B,)):
+            raise ValueError(f"inputs['speaker'] must be a contiguous int32 CUDA tensor of shape [{B}], got "
+                             f"{spk.dtype} {spk.device} {tuple(spk.shape)}")
+        table = self.store["speaker/embed"]
+        e = self.runtime.buf("speaker/e", (B, table.shape[1]))
+        L.check(L.lib().taco_gather_rows(L.ptr(table), L.ptr(spk), B, table.shape[1], table.shape[0], None, 1.0, L.ptr(e),
+                                         L.current_stream()), "taco_gather_rows")
+        return e
+
     def _encoder(self, inputs, train, enc_drop_masks, trace):
         cfg, store = self.config, self.store
+        speaker_embed = self._speaker_embed(inputs)
         # embedding lookup fused with the first pre-net layer (tacotron.py:111-114, :128)
         with ops.variable_scope(store, "enc"):
             pre_out = self.pre_net(store["embedding"], dropout=cfg.char_dropout_prob, train=train, masks=enc_drop_masks,
                                    ids=inputs["text"])
-            encoded = ops.CBHG(pre_out, None, K=16, c=[128, 128, 128], gru_units=128, trace=trace)      # :131
+            encoded = ops.CBHG(pre_out, speaker_embed, K=16, c=[128, 128, 128], gru_units=128, trace=trace)   # :131
         if trace is not None:
             trace["enc/prenet_out"] = pre_out
             trace["encoded"] = encoded
@@ -192,6 +211,9 @@ class Tacotron(object):
             if not hasattr(self, "_graphs"):
                 self._graphs = {}
             static = {"text": inputs["text"].clone(), "text_length": inputs["text_length"].clone()}
+            if self.config.num_speakers > 1:
+                self._speaker_embed(inputs)                         # validates the ids before they are captured
+                static["speaker"] = inputs["speaker"].clone()
             marks, self._marks = self._marks, None
             cg_flag, self.config.cuda_graph = self.config.cuda_graph, False
             try:
@@ -220,6 +242,10 @@ class Tacotron(object):
         static, graphs, outs, _ = g
         static["text"].copy_(inputs["text"], non_blocking=True)
         static["text_length"].copy_(inputs["text_length"], non_blocking=True)
+        if "speaker" in static:
+            if inputs.get("speaker") is None:
+                raise ValueError(f"a model with num_speakers = {self.config.num_speakers} needs inputs['speaker'] (int32 [B])")
+            static["speaker"].copy_(inputs["speaker"], non_blocking=True)
         # optional events a pipelined caller sets so that a section does not overwrite a result buffer that an
         # asynchronous device->host copy of the PREVIOUS call is still reading (bench.py e2e)
         waits = getattr(self, "section_wait", None) or {}
@@ -307,6 +333,8 @@ class Tacotron(object):
             self.seq2seq_output, self.output = self.inference(inputs, True, **kw)
         self.loss = self.add_loss_op(self.seq2seq_output, self.output, inputs["mel"], inputs["stft"])
         S.update(text=inputs["text"], text_length=inputs["text_length"], mel=inputs["mel"], stft=inputs["stft"])
+        if self.config.num_speakers > 1:
+            S["speaker"] = inputs["speaker"]
         S["post/out"] = self.output
         self.saved = S
         self.backward(S)

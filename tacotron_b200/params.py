@@ -72,6 +72,21 @@ def model_shapes(cfg):
     P += [("dec/out_proj/W", (U, mel_out), "dense"), ("dec/out_proj/b", (mel_out,), "zeros")]
     P += cbhg_shapes("post/cbhg", cfg.mel_features, 8, (128, 256, 80))
     P += [("post/dense/W", (256, cfg.fft_size), "dense"), ("post/dense/b", (cfg.fft_size,), "zeros")]
+    if getattr(cfg, "num_speakers", 1) > 1:
+        P += speaker_shapes(cfg.num_speakers, getattr(cfg, "speaker_embed_dim", 16))
+    return P
+
+
+def speaker_shapes(num_speakers, E=16, n_hw=4, units=128):
+    """Multi-speaker variables (tacotron.py:116-124, ops.py:101-115), stored after the single-speaker ones so that the
+    layout of those does not depend on the speaker count: the speaker table; per encoder highway layer the speaker dense
+    Ws/bs (E -> 128, relu) and the width-fixing dense Wd/bd of the [h | s] input (256 -> 128, ops.py:29-30); the dense
+    gru_init/Ws,bs giving the initial state of both bi-GRU directions."""
+    P = [("speaker/embed", (num_speakers, E), "dense")]
+    for l in range(n_hw):
+        P += [(f"enc/cbhg/highway{l}/Ws", (E, units), "dense"), (f"enc/cbhg/highway{l}/bs", (units,), "zeros"),
+              (f"enc/cbhg/highway{l}/Wd", (2 * units, units), "dense"), (f"enc/cbhg/highway{l}/bd", (units,), "zeros")]
+    P += [("enc/cbhg/gru_init/Ws", (E, units), "dense"), ("enc/cbhg/gru_init/bs", (units,), "zeros")]
     return P
 
 

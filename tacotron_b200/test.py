@@ -1,6 +1,7 @@
 """Synthesis driver -- eager equivalent of the reference's ``test.py`` (test.py:13-88; SURVEY.md section 8(f) rank 2).
 
     echo "a prompt to say" | python -m tacotron_b200.test -t nancy
+    echo "a prompt to say" | python -m tacotron_b200.test -t vctk -s 3      # multi-speaker model: speaker id 3
 
 Prompts come from stdin, one per line (test.py:77-78); they are encoded and padded to 140 characters exactly as
 ``data_input.load_prompts`` does (quirks included), run through ``Tacotron.inference`` in batches of at most 32, every
@@ -18,7 +19,7 @@ import numpy as np
 import torch
 
 
-def test(model_cls, config, prompts, log=print):
+def test(model_cls, config, prompts, log=print, speaker=0):
     from . import audio, checkpoint, data_input
     from .train import write_wav
     sr = 24000 if "blizzard" in config.data_path else 16000                              # test.py:15
@@ -28,11 +29,10 @@ def test(model_cls, config, prompts, log=print):
     ivocab = meta["vocab"]
     config.vocab_size = len(ivocab)                                                      # :19
     config.num_prompts = len(prompts)                                                    # :23
-    model = model_cls(config, None, train=False)                                         # :31
-    log("restoring weights")                                                             # :41
     ck = checkpoint.latest_checkpoint(os.path.join("weights", config.save_path))         # :42-45
+    tf_ck = None
     if ck is not None:
-        stft_mean, stft_std = checkpoint.restore(model, ck)                              # :46-48
+        config.num_speakers = checkpoint.num_speakers(ck)
     else:
         # no checkpoint of ours: a checkpoint written by the reference itself (TensorFlow V2 format, e.g. the released
         # Nancy weights of download_weights.sh) in the same directory is read directly
@@ -40,6 +40,15 @@ def test(model_cls, config, prompts, log=print):
         tf_ck = tf_checkpoint.latest_checkpoint(os.path.dirname(os.path.join("weights", config.save_path)))
         if tf_ck is None:
             raise FileNotFoundError(f"no checkpoint under weights/{config.save_path}")
+        spk = tf_checkpoint.read_bundle(tf_ck, names={"speaker/speaker_embed"}).get("speaker/speaker_embed")
+        config.num_speakers = 1 if spk is None else int(np.asarray(spk).shape[0])
+    if not 0 <= speaker < config.num_speakers:
+        raise ValueError(f"speaker id {speaker} out of range: the checkpoint has {config.num_speakers} speaker(s)")
+    model = model_cls(config, None, train=False)                                         # :31
+    log("restoring weights")                                                             # :41
+    if ck is not None:
+        stft_mean, stft_std = checkpoint.restore(model, ck)                              # :46-48
+    else:
         extra = checkpoint.import_tf_checkpoint(model, tf_ck)
         stft_mean, stft_std = extra["stft_mean"], extra["stft_std"]
     mean_d = torch.from_numpy(np.asarray(stft_mean, dtype=np.float32)).cuda()
@@ -49,6 +58,8 @@ def test(model_cls, config, prompts, log=print):
     n = 0
     waves = []
     for inputs in data_input.load_prompts(prompts, ivocab):                              # :21-22, :50-56
+        if config.num_speakers > 1:
+            inputs["speaker"] = torch.full((inputs["text"].shape[0],), speaker, dtype=torch.int32, device=inputs["text"].device)
         _, outputs = model.inference(inputs, train=False)
         alignments = model.alignments
         log("saving samples")
@@ -67,6 +78,7 @@ def test(model_cls, config, prompts, log=print):
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", "--train-set", default="nancy")
+    parser.add_argument("-s", "--speaker", type=int, default=0, help="speaker id of a multi-speaker model")
     args = parser.parse_args(argv)
     prompts = [p for p in sys.stdin.readlines() if len(p) > 0]                           # test.py:77-78
     from .models.tacotron import Config, Tacotron
@@ -74,7 +86,7 @@ def main(argv=None):
     config.data_path = "data/%s/" % args.train_set                                       # :83
     config.save_path = args.train_set + "/tacotron"                                      # :84
     print("Building Tacotron")
-    test(Tacotron, config, prompts)
+    test(Tacotron, config, prompts, speaker=args.speaker)
 
 
 if __name__ == "__main__":

@@ -8,13 +8,16 @@ tensors keep their TF layouts (dense [in,out], conv [k,Cin,Cout], GRU gates/cand
 import re
 
 
-def tf_name_to_param(name):
+def tf_name_to_param(name, multi_speaker=False):
     """TF-1.2-style variable name -> parameter name of tacotron_b200.params (same layouts, so a checkpoint tensor
     can be copied as is).  Raises KeyError for variables that are not part of the model (global_step, Adam slots,
-    stft_mean/std, ...)."""
+    stft_mean/std, ...).  multi_speaker: the graph of a model with num_speakers > 1 (tacotron.py:116-124,
+    ops.py:101-115), whose encoder highway layers open with a speaker dense and a width-fixing dense."""
     import re
     if name == "embedding/embedding":
         return "embedding"
+    if multi_speaker and name == "speaker/speaker_embed":
+        return "speaker/embed"
     kb = {"kernel": "W", "bias": "b"}
     m = re.match(r"(encoder|decoder/decoder/attention_wrapper)/pre_net/dense(_1)?/(kernel|bias)$", name)
     if m:
@@ -38,9 +41,14 @@ def tf_name_to_param(name):
         mm = re.match(r"highway_(\d+)/dense(?:_(\d+))?/(kernel|bias)$", rest)
         if mm:
             l, j = int(mm.group(1)), int(mm.group(2) or 0)
-            has_fix = (pre == "post/cbhg" and l == 0)          # ops.py:29-30: extra dense when the width != 128
-            role = (["d", "T", "H"] if has_fix else ["T", "H"])[j]
+            if multi_speaker and pre == "enc/cbhg":            # speaker dense, then the 256 -> 128 width fix (ops.py:101-107)
+                role = ["s", "d", "T", "H"][j]
+            else:
+                has_fix = (pre == "post/cbhg" and l == 0)      # ops.py:29-30: extra dense when the width != 128
+                role = (["d", "T", "H"] if has_fix else ["T", "H"])[j]
             return f"{pre}/highway{l}/{kb[mm.group(3)]}{role}"
+        if multi_speaker and pre == "enc/cbhg" and rest in ("dense/kernel", "dense/bias"):   # bi-GRU initial state (ops.py:111-115)
+            return f"{pre}/gru_init/{kb[rest.rsplit('/', 1)[1]]}s"
         mm = re.match(r"bidirectional_rnn/(fw|bw)/gru_cell/(gates|candidate)/(kernel|bias)$", rest)
         if mm:
             return f"{pre}/gru_{mm.group(1)}/{kb[mm.group(3)]}{'g' if mm.group(2) == 'gates' else 'c'}"
