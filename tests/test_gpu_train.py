@@ -61,7 +61,9 @@ def test_model_backward_matches_autograd(r, sched):
 @pytest.mark.parametrize("r,sched", [(2, True), (5, False)])
 def test_model_backward_fp32x3_matches_autograd(r, sched):
     """the default precision mode: 3xTF32 wgmma forward, data gradients on the same wgmma kernel (3xTF32), weight gradients on
-    the 3xTF32 mma.sync GEMM -- held to the SAME bars as the exact-product fp32 mode"""
+    the 3xTF32 mma.sync GEMM -- held to the SAME bars as the exact-product fp32 mode.  (At this toy size every product stays
+    below kernels.DW_TC_MIN_ROWS / GEMM_TC_MIN_ROWS; the taco_conv_dw and wgmma-product routes the benchmark's training step
+    takes are checked in test_gpu_train_fullsize.py.)"""
     res = TC.check_model_bwd(r, sched, "fp32x3")
     # The 3xTF32 forward differs from the fp32 oracle by ~1e-6, enough to put an occasional unit on the other side of a
     # derivative discontinuity (relu mask, max-pool argmax, sign() of the L1 loss).  scripts/debug/bwd_matrix.py shows it:

@@ -30,7 +30,16 @@ def test_saving_forward_matches_oracle(r, sched):
 
 @pytest.mark.parametrize("r,sched", [(2, True), (5, False), (5, True)])
 def test_backward_matches_autograd(r, sched):
-    cfg, p, inp, enc_m, dec_m, sm = _setup(r, sched)
+    _check_backward_against_autograd(*_setup(r, sched))
+
+
+def test_backward_matches_autograd_batch_sized():
+    """a batch of 32 ragged utterances, Tx = 67 (not a multiple of 4, 8 or 32), T = 64, scheduled sampling: the float64
+    mirror backward is the reference of tests/test_gpu_train_fullsize.py, so it is pinned here beyond the toy shape"""
+    _check_backward_against_autograd(*_setup(5, True, B=32, Tx=67, T=64))
+
+
+def _check_backward_against_autograd(cfg, p, inp, enc_m, dec_m, sm):
     loss, g_ref = O.loss_and_grads(p, inp, cfg, enc_drop_masks=enc_m, dec_drop_masks=dec_m, sample_mask=sm)
     S, y, out = grad_util.saving_forward(p, inp, cfg, enc_m, dec_m, sm)
     G = {k: torch.zeros_like(v) for k, v in p.items()}
