@@ -331,6 +331,30 @@ int taco_irfft2048(float* x, const float* X_c64, int64_t rows, void* stream);
 int taco_normalize_f16(float* out, const void* x_f16, const void* mean_f16, const float* std_f32, int64_t rows, int W,
                        void* stream);
 
+/* ==========================================================================================
+ * Feature extraction (preprocess.py:168-208 / audio.py:38-65): WAV samples -> the float16 training arrays.  The
+ * waveforms of a chunk are packed end to end (fp32) with int64 offsets; the transform between the two feature kernels is
+ * taco_rfft2048.  Semantics: tests/mirror_kernels_features.py.
+ * ========================================================================================== */
+/* librosa.effects.trim (audio.py:42): one CTA per utterance b = samples [offsets[b], offsets[b+1]).  Frame f < 1 + len/hop
+ * of the signal reflect-padded by frame_length/2 has mean-square energy e_f (fp64); it is non-silent when
+ * 10 log10(max(1e-10, e_f)) - 10 log10(max(1e-10, max e)) > -top_db.  bounds[b] = {first*hop, min(len, (last+1)*hop)}
+ * relative to offsets[b], {0, 0} if no frame is non-silent.  frame_length an even multiple of hop, at most 16 hops;
+ * each utterance longer than frame_length/2.                                                                        */
+int taco_trim_bounds(int* bounds, const float* y, const int64_t* offsets, int B, int frame_length, int hop, float top_db,
+                     void* stream);
+/* head of librosa.stft after trimming (audio.py:47-56): w_b = y[start[b] : start[b]+len[b]] zero-padded to max_len
+ * (len[b] <= max_len), pre-emphasis e[0] = w[0], e[i] = w[i] - preemph*w[i-1] (fp32, two roundings), reflect padding by
+ * n_fft/2, framing, hann window: frw [B][n_frames][n_fft], n_frames = 1 + max_len/hop.                                 */
+int taco_feature_frames(float* frw, const float* y, const int64_t* start, const int* len, int B, int n_frames, int max_len,
+                        int hop, int n_fft, int win_length, float preemph, void* stream);
+/* audio.py:57-63 from X [B][n_frames][1025] complex (taco_rfft2048): stft = log(|X| + 1e-8), mel[m] = log(|sum_{k in
+ * [mel_lo[m], mel_hi[m])} mel_basis[m][k] X[k]| + 1e-8) (mel_basis [n_mels][1025]; 0 <= lo <= hi <= 1025), scattered in
+ * the reshape_frames(forward=True) layout: stft_out [B][4*(n_frames/4r)][1025 r], mel_out [B][..][n_mels r], float16
+ * (out_f16 = 1) or float32.  Frames beyond 4r*(n_frames/4r) are not written.                                        */
+int taco_feature_spec(void* stft_out, void* mel_out, int out_f16, const float* X_c64, const float* mel_basis, const int* mel_lo,
+                      const int* mel_hi, int B, int n_frames, int r, int n_mels, void* stream);
+
 int taco_sumsq(const float* x, int64_t n, float* partial_ws, float* out, void* stream);
 int taco_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr_t, float b1, float b2, float eps,
                    float clip, const float* sumsq, void* stream);

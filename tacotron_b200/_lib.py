@@ -105,6 +105,8 @@ EXPORTS = [
     "taco_gl_init", "taco_gl_ola", "taco_gl_frame", "taco_gl_phase", "taco_rfft2048", "taco_irfft2048",
     # input data format
     "taco_normalize_f16",
+    # feature extraction (preprocessing)
+    "taco_trim_bounds", "taco_feature_frames", "taco_feature_spec",
 ]
 
 
@@ -170,6 +172,9 @@ def lib():
     L.taco_rfft2048.argtypes = [vp, vp, i64, vp]
     L.taco_irfft2048.argtypes = [vp, vp, i64, vp]
     L.taco_normalize_f16.argtypes = [vp, vp, vp, vp, i64, i32, vp]
+    L.taco_trim_bounds.argtypes = [vp, vp, vp, i32, i32, i32, f32, vp]
+    L.taco_feature_frames.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.taco_feature_spec.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     for name in EXPORTS:                      # every declared symbol must resolve (AttributeError otherwise)
         getattr(L, name)
     _lib = L

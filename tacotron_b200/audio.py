@@ -14,9 +14,15 @@ round 1 called cuFFT through ``torch.fft`` here); everything between them is fou
 so one iteration is irfft2048 -> gl_ola -> gl_frame -> rfft2048 -> gl_phase: 5 launches of this library, ~20 MB of HBM traffic per utterance of
 500 frames.  All arithmetic goes through the kernel namespace K (tacotron_b200/kernels.py); tests run the same
 orchestration over tests/mirror_kernels.py on CPU tensors against the numpy oracle (oracle/audio_oracle.py).
+
+Feature extraction (the reference's ``process_audio``, audio.py:38-65, used by tacotron_b200/preprocess.py) is the
+analysis half of the same transform: trim_bounds -> feature_frames -> rfft2048 -> feature_spec, four launches per chunk of
+utterances (csrc/features.cu).  ``load_wav`` reads a WAV file the way ``librosa.load(f, mono=True, sr=sr)`` does when no
+resampling is needed; a file at another rate is an error, since resampling is not implemented.
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 n_fft = 2048            # audio.py:10
@@ -24,6 +30,135 @@ win_length = 1200       # audio.py:11
 hop_length = 300        # audio.py:12
 maximum_audio_length = 108000   # audio.py:13
 F_BINS = 1 + n_fft // 2
+PRE_EMPHASIS = 0.97     # audio.py:53
+N_MELS = 80             # audio.py:57
+MEL_SR = 22050          # librosa's default sr: melspectrogram(S=stft) builds its basis at this rate, not the file's
+TRIM_TOP_DB, TRIM_FRAME, TRIM_HOP = 60.0, 2048, 512     # librosa.effects.trim defaults (audio.py:42)
+STFT_FRAMES = 1 + maximum_audio_length // hop_length     # 361
+MIN_SAMPLES = n_fft // 2 + 1                             # shorter signals cannot be reflect-padded by n_fft/2
+
+
+def feature_frames_per_utterance(r):
+    """rows of the stored arrays: 4*(361 // 4r) frames survive reshape_frames; the reference allocates
+    maximum_audio_length // (hop*r) rows (preprocess.py:178).  The two agree for r in {1, 2, 3, 5, 6}.  At r = 4 they
+    do not (88 vs 90), and the reference fails on the assignment (preprocess.py:194); its guard (audio.py:46) never
+    fires because `% 4*r` is `(x % 4) * r`."""
+    if r < 1:
+        raise ValueError(f"r = {r} is not supported for preprocessing (use r in 1, 2, 3, 5, 6)")
+    rows, stored = 4 * (STFT_FRAMES // (4 * r)), maximum_audio_length // (hop_length * r)
+    if rows != stored:
+        raise ValueError(f"r = {r} is not supported for preprocessing: reshape_frames keeps {rows} rows of "
+                         f"{maximum_audio_length} samples, but the stored arrays have {stored} (use r in 1, 2, 3, 5, 6)")
+    return rows
+
+
+def load_wav(path, sr):
+    """librosa.load(path, mono=True, sr=sr) (audio.py:39) for a WAV file already at `sr`: float32 samples (int16 / 32768,
+    int32 and 24-bit / 2^31, (uint8 - 128) / 128, float as stored), channels averaged in float32."""
+    from scipy.io import wavfile
+    rate, x = wavfile.read(path)
+    if rate != sr:
+        raise ValueError(f"{path}: sample rate {rate} Hz, expected {sr} Hz (resampling is not supported)")
+    if x.dtype == np.int16:
+        x = x.astype(np.float32) / np.float32(32768.0)
+    elif x.dtype == np.int32:
+        x = (x.astype(np.float64) / 2147483648.0).astype(np.float32)
+    elif x.dtype == np.uint8:
+        x = (x.astype(np.float32) - np.float32(128.0)) / np.float32(128.0)
+    elif x.dtype.kind == "f":
+        x = x.astype(np.float32)
+    else:
+        raise ValueError(f"{path}: unsupported WAV sample format {x.dtype}")
+    if x.ndim == 2:
+        x = np.mean(x, axis=1, dtype=np.float32)
+    return np.ascontiguousarray(x)
+
+
+def mel_basis(sr=MEL_SR, n_mels=N_MELS):
+    """librosa.filters.mel(sr, n_fft=2048, n_mels, dtype=float32) (librosa 0.6-0.9: Slaney mel scale, fmin 0, fmax sr/2,
+    norm=1) -> basis float32 [n_mels, 1025] and the range [lo, hi) of bins each filter covers (int32 [n_mels] each).
+    Each row is rounded to float32, then scaled by the area normalisation in float64 and rounded again, as librosa's
+    in-place `weights *= enorm` does."""
+    f_sp, min_log_hz = 200.0 / 3, 1000.0
+    min_log_mel, logstep = min_log_hz / f_sp, np.log(6.4) / 27.0
+
+    def hz_to_mel(f):
+        return min_log_mel + np.log(f / min_log_hz) / logstep if f >= min_log_hz else f / f_sp
+
+    mels = np.linspace(hz_to_mel(0.0), hz_to_mel(sr / 2.0), n_mels + 2)
+    mel_f = np.where(mels >= min_log_mel, min_log_hz * np.exp(logstep * (mels - min_log_mel)), f_sp * mels)
+    fftfreqs = np.linspace(0, sr / 2.0, F_BINS, endpoint=True)
+    fdiff = np.diff(mel_f)
+    ramps = np.subtract.outer(mel_f, fftfreqs)
+    weights = np.zeros((n_mels, F_BINS), dtype=np.float32)
+    for i in range(n_mels):
+        weights[i] = np.maximum(0, np.minimum(-ramps[i] / fdiff[i], ramps[i + 2] / fdiff[i + 1]))
+    weights *= (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]
+    lo = np.zeros(n_mels, dtype=np.int32)
+    hi = np.zeros(n_mels, dtype=np.int32)
+    for i in range(n_mels):
+        nz = np.flatnonzero(weights[i])
+        if nz.size:
+            lo[i], hi[i] = nz[0], nz[-1] + 1
+    return weights, lo, hi
+
+
+_mel_dev = {}
+
+
+def _mel_on(device):
+    key = str(device)
+    if key not in _mel_dev:
+        _mel_dev[key] = tuple(torch.from_numpy(a).to(device) for a in mel_basis())
+    return _mel_dev[key]
+
+
+def process_audio_batch(waves, r, K=None, device="cuda", out_dtype=torch.float16):
+    """The reference's process_audio (audio.py:38-65) for a chunk of mono float32 waveforms (numpy, each at least
+    1025 samples): trim silence, drop an utterance longer than maximum_audio_length after trimming, zero-pad, pre-emphasise,
+    STFT, mel, log, reshape_frames(forward=True).  Returns (mel [n, T, 80 r], stft [n, T, 1025 r], keep [N] bool) with
+    the n = keep.sum() kept utterances in order, T = feature_frames_per_utterance(r); the arrays are on `device`."""
+    K = K or _K()
+    T = feature_frames_per_utterance(r)
+    lens = np.array([len(w) for w in waves], dtype=np.int64)
+    short = np.flatnonzero(lens < MIN_SAMPLES)
+    if short.size:
+        raise ValueError(f"utterance {int(short[0])} has {int(lens[short[0]])} samples; at least {MIN_SAMPLES} are needed")
+    N = len(waves)
+    offsets = np.zeros(N + 1, dtype=np.int64)
+    np.cumsum(lens, out=offsets[1:])
+    cuda = torch.device(device).type == "cuda"
+    y = torch.from_numpy(np.concatenate(waves).astype(np.float32, copy=False) if N else np.zeros(0, np.float32))
+    y = (y.pin_memory() if cuda else y).to(device, non_blocking=True)
+    bounds = torch.empty((N, 2), dtype=torch.int32, device=device)
+    K.trim_bounds(bounds, y, torch.from_numpy(offsets).to(device), TRIM_FRAME, TRIM_HOP, TRIM_TOP_DB)
+    b = bounds.cpu().numpy().astype(np.int64)
+    kept_len = b[:, 1] - b[:, 0]
+    keep = kept_len <= maximum_audio_length
+    idx = np.flatnonzero(keep)
+    n = len(idx)
+    mel = torch.empty((n, T, N_MELS * r), dtype=out_dtype, device=device)
+    stft = torch.empty((n, T, F_BINS * r), dtype=out_dtype, device=device)
+    if n:
+        start = torch.from_numpy(offsets[idx] + b[idx, 0]).to(device)
+        length = torch.from_numpy(kept_len[idx].astype(np.int32)).to(device)
+        frw = torch.empty((n, STFT_FRAMES, n_fft), dtype=torch.float32, device=device)
+        K.feature_frames(frw, y, start, length, maximum_audio_length, hop_length, win_length, PRE_EMPHASIS)
+        X = torch.empty((n, STFT_FRAMES, F_BINS), dtype=torch.complex64, device=device)
+        K.rfft2048(X, frw)
+        del frw
+        basis, lo, hi = _mel_on(device)
+        K.feature_spec(stft, mel, X, basis, lo, hi, r)
+    return mel, stft, keep
+
+
+def process_audio(fname, sr=16000, r=2, K=None, device="cuda"):
+    """audio.process_audio(fname, sr=sr) (audio.py:38-65) with r explicit: (mel [T, 80 r], stft [T, 1025 r]) float16 numpy
+    arrays, or (None, None) when the trimmed utterance is longer than maximum_audio_length."""
+    mel, stft, keep = process_audio_batch([load_wav(fname, sr)], r, K=K, device=device)
+    if not keep[0]:
+        return None, None
+    return mel[0].cpu().numpy(), stft[0].cpu().numpy()
 
 
 def _K():

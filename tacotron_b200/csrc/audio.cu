@@ -18,12 +18,6 @@ inline int grid_for(int64_t total, int block) {
     return (int)g;
 }
 
-__device__ __forceinline__ float hann_at(int j, int lpad, int win_length) {   // j in [0, n_fft); 0 outside the support
-    const int i = j - lpad;
-    if (i < 0 || i >= win_length) return 0.f;
-    return 0.5f - 0.5f * cospif(2.0f * (float)i / (float)win_length);
-}
-
 // mag[b,f,k] = exp(spec[b, t(f), c(f)*F + k] * scale + shift);  full = mag * exp(2 pi i u)
 __global__ void gl_init_kernel(float2* __restrict__ full, float* __restrict__ mag, const float* __restrict__ spec,
                                const float* __restrict__ phase_u, int T, int n, int r, int F, const float* __restrict__ scale,

@@ -70,6 +70,13 @@ __device__ __forceinline__ float tanhf_acc(float x) {
     float e = __expf(2.0f * x);
     return 1.0f - __fdividef(2.0f, e + 1.0f);
 }
+// periodic hann window of win_length samples centred in the n_fft-sample frame (lpad = (n_fft - win_length)/2), as
+// librosa's stft / istft build it; j in [0, n_fft), 0 outside the support
+__device__ __forceinline__ float hann_at(int j, int lpad, int win_length) {
+    const int i = j - lpad;
+    if (i < 0 || i >= win_length) return 0.f;
+    return 0.5f - 0.5f * cospif(2.0f * (float)i / (float)win_length);
+}
 __device__ __forceinline__ float apply_act(float v, int act) {
     switch (act) {
         case TACO_ACT_RELU:    return fmaxf(v, 0.0f);

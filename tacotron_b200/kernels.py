@@ -403,6 +403,48 @@ def normalize_f16(out, x, mean, std):
     L.check(L.lib().taco_normalize_f16(_p(out), _p(x), _p(mean), _p(std), x.numel() // W, W, _st()), "taco_normalize_f16")
 
 
+# ---- feature extraction (tacotron_b200/audio.py process_audio_batch) ----
+def _cuda_c(t, dtype, name):
+    if not (t.is_cuda and t.is_contiguous() and t.dtype == dtype):
+        raise L.TacoError(f"{name}: expected a contiguous CUDA {dtype} tensor, got {t.dtype} {t.device}")
+    return t
+
+
+def trim_bounds(bounds, y, offsets, frame_length, hop, top_db):
+    """bounds int32 [B, 2] = librosa.effects.trim's kept span of each utterance y[offsets[b]:offsets[b+1]] (fp32 y)"""
+    B = offsets.numel() - 1
+    _cuda_c(bounds, torch.int32, "trim_bounds bounds"); _cuda_c(y, torch.float32, "trim_bounds y")
+    _cuda_c(offsets, torch.int64, "trim_bounds offsets")
+    assert bounds.shape == (B, 2)
+    L.check(L.lib().taco_trim_bounds(_p(bounds), _p(y), _p(offsets), B, frame_length, hop, float(top_db), _st()), "taco_trim_bounds")
+
+
+def feature_frames(frw, y, start, length, max_len, hop, win_length, preemph):
+    """frw fp32 [B, n, n_fft] = windowed frames of the pre-emphasised, zero-padded span y[start[b]:start[b]+length[b]]"""
+    B, n, n_fft = frw.shape
+    _f32c(frw, "feature_frames frw"); _cuda_c(y, torch.float32, "feature_frames y")
+    _cuda_c(start, torch.int64, "feature_frames start"); _cuda_c(length, torch.int32, "feature_frames length")
+    assert start.shape == (B,) and length.shape == (B,)
+    L.check(L.lib().taco_feature_frames(_p(frw), _p(y), _p(start), _p(length), B, n, max_len, hop, n_fft, win_length,
+                                        float(preemph), _st()), "taco_feature_frames")
+
+
+def feature_spec(stft_out, mel_out, X, basis, lo, hi, r):
+    """log |X| and log |basis . X| of X complex64 [B, n, 1025] in the reshape_frames layout: stft_out [B, T, 1025 r],
+    mel_out [B, T, n_mels r], both float16 or both float32"""
+    B, n, F = X.shape
+    n_mels = basis.shape[0]
+    f16 = stft_out.dtype == torch.float16
+    for t, nm in ((stft_out, "stft_out"), (mel_out, "mel_out")):
+        _cuda_c(t, torch.float16 if f16 else torch.float32, f"feature_spec {nm}")
+    _cuda_c(X, torch.complex64, "feature_spec X"); _cuda_c(basis, torch.float32, "feature_spec basis")
+    _cuda_c(lo, torch.int32, "feature_spec lo"); _cuda_c(hi, torch.int32, "feature_spec hi")
+    T = 4 * (n // (4 * r))
+    assert F == 1025 and basis.shape == (n_mels, F) and stft_out.shape == (B, T, F * r) and mel_out.shape == (B, T, n_mels * r)
+    L.check(L.lib().taco_feature_spec(_p(stft_out), _p(mel_out), int(f16), _p(X), _p(basis), _p(lo), _p(hi), B, n, r, n_mels,
+                                      _st()), "taco_feature_spec")
+
+
 _ss_ws = {}
 
 
