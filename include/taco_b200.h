@@ -354,6 +354,16 @@ int taco_feature_frames(float* frw, const float* y, const int64_t* start, const 
  * (out_f16 = 1) or float32.  Frames beyond 4r*(n_frames/4r) are not written.                                        */
 int taco_feature_spec(void* stft_out, void* mel_out, int out_f16, const float* X_c64, const float* mel_basis, const int* mel_lo,
                       const int* mel_hi, int B, int n_frames, int r, int n_mels, void* stream);
+/* the resampling of librosa.load(f, sr=sr) (audio.py:39) for files at another rate: librosa 0.6 resample(res_type=
+ * 'kaiser_best') over resampy 0.2.2's loop, one ratio = sr_new / sr_orig per call.  Input b = in[in_off[b] : in_off[b+1]]
+ * (n_in samples), output b = out[out_off[b] : out_off[b+1]] (librosa's n_fix = ceil(n_in*ratio) samples): the first
+ * n_out = int(n_in*ratio) samples are resampy's, the rest zeros.  win_delta [nwin][2] float64 = {win, delta} of the
+ * (ratio-scaled) 512-entries-per-crossing table, 16-byte aligned; step = int(min(1, ratio)*512); treg [treg_len] the
+ * float64 time register (treg[t] = treg[t-1] + 1/ratio, summed in order), treg_len >= every n_out (an output sample the
+ * register does not reach is written as NaN).  Float32 accumulation rounded after every tap, no fused multiply-add:
+ * bit-identical to tests/mirror_kernels_resample.py.  B <= 65535.                                                   */
+int taco_resample(float* out, const float* in, const int64_t* in_off, const int64_t* out_off, int B, const double* win_delta,
+                  int nwin, int step, double ratio, const double* treg, int64_t treg_len, void* stream);
 
 int taco_sumsq(const float* x, int64_t n, float* partial_ws, float* out, void* stream);
 int taco_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr_t, float b1, float b2, float eps,

@@ -106,7 +106,7 @@ EXPORTS = [
     # input data format
     "taco_normalize_f16",
     # feature extraction (preprocessing)
-    "taco_trim_bounds", "taco_feature_frames", "taco_feature_spec",
+    "taco_trim_bounds", "taco_feature_frames", "taco_feature_spec", "taco_resample",
 ]
 
 
@@ -175,6 +175,7 @@ def lib():
     L.taco_trim_bounds.argtypes = [vp, vp, vp, i32, i32, i32, f32, vp]
     L.taco_feature_frames.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
     L.taco_feature_spec.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    L.taco_resample.argtypes = [vp, vp, vp, vp, i32, vp, i32, i32, C.c_double, vp, i64, vp]
     for name in EXPORTS:                      # every declared symbol must resolve (AttributeError otherwise)
         getattr(L, name)
     _lib = L

@@ -18,9 +18,13 @@ orchestration over tests/mirror_kernels.py on CPU tensors against the numpy orac
 Feature extraction (the reference's ``process_audio``, audio.py:38-65, used by tacotron_b200/preprocess.py) is the
 analysis half of the same transform: trim_bounds -> feature_frames -> rfft2048 -> feature_spec, four launches per chunk of
 utterances (csrc/features.cu).  ``load_wav`` reads a WAV file the way ``librosa.load(f, mono=True, sr=sr)`` does when no
-resampling is needed; a file at another rate is an error, since resampling is not implemented.
+resampling is needed and rejects a file at another rate.  ``read_wav`` returns the file's rate instead, and
+``resample_batch`` / ``process_audio_batch(rates=...)`` do librosa.load's resampling on the device (csrc/resample.cu:
+librosa 0.6's kaiser_best over resampy 0.2.2's loop, one launch per source rate in a chunk).
 """
 from __future__ import annotations
+
+import functools
 
 import numpy as np
 import torch
@@ -36,6 +40,8 @@ MEL_SR = 22050          # librosa's default sr: melspectrogram(S=stft) builds it
 TRIM_TOP_DB, TRIM_FRAME, TRIM_HOP = 60.0, 2048, 512     # librosa.effects.trim defaults (audio.py:42)
 STFT_FRAMES = 1 + maximum_audio_length // hop_length     # 361
 MIN_SAMPLES = n_fft // 2 + 1                             # shorter signals cannot be reflect-padded by n_fft/2
+RS_ZEROS, RS_TABLE = 64, 512                             # resampy's kaiser_best: 64 zero crossings, 2^9 entries each
+RS_BETA, RS_ROLLOFF = 14.769656459379492, 0.9475937167399596
 
 
 def feature_frames_per_utterance(r):
@@ -53,12 +59,20 @@ def feature_frames_per_utterance(r):
 
 
 def load_wav(path, sr):
-    """librosa.load(path, mono=True, sr=sr) (audio.py:39) for a WAV file already at `sr`: float32 samples (int16 / 32768,
-    int32 and 24-bit / 2^31, (uint8 - 128) / 128, float as stored), channels averaged in float32."""
+    """librosa.load(path, mono=True, sr=sr) (audio.py:39) for a WAV file already at `sr` (see read_wav); a file at another
+    rate is an error (read_wav + resample_batch convert it)."""
+    x, rate = read_wav(path)
+    if rate != sr:
+        raise ValueError(f"{path}: sample rate {rate} Hz, expected {sr} Hz (load_wav does not resample; preprocess with "
+                         f"--resample to convert it)")
+    return x
+
+
+def read_wav(path):
+    """a WAV file as librosa.load(path, mono=True, sr=None) reads it -> (float32 samples, rate): int16 / 32768, int32 and
+    24-bit / 2^31, (uint8 - 128) / 128, float as stored, channels averaged in float32."""
     from scipy.io import wavfile
     rate, x = wavfile.read(path)
-    if rate != sr:
-        raise ValueError(f"{path}: sample rate {rate} Hz, expected {sr} Hz (resampling is not supported)")
     if x.dtype == np.int16:
         x = x.astype(np.float32) / np.float32(32768.0)
     elif x.dtype == np.int32:
@@ -71,7 +85,116 @@ def load_wav(path, sr):
         raise ValueError(f"{path}: unsupported WAV sample format {x.dtype}")
     if x.ndim == 2:
         x = np.mean(x, axis=1, dtype=np.float32)
-    return np.ascontiguousarray(x)
+    return np.ascontiguousarray(x), int(rate)
+
+
+def resample_lengths(n_in, sr_orig, sr_new, what="signal"):
+    """(n_out, n_fix) of librosa.resample: resampy computes int(n_in * ratio) samples (fewer than one is an error naming
+    `what`), librosa zero-pads them to ceil(n_in * ratio)"""
+    ratio = float(sr_new) / sr_orig
+    n_out, n_fix = int(n_in * ratio), int(np.ceil(n_in * ratio))
+    if n_out < 1:
+        raise ValueError(f"{what}: {n_in} samples at {sr_orig} Hz are too few to resample to {sr_new} Hz")
+    return n_out, n_fix
+
+
+@functools.lru_cache(maxsize=None)
+def _kaiser_best():
+    from scipy.signal.windows import kaiser
+    n = RS_TABLE * RS_ZEROS
+    return kaiser(2 * n + 1, RS_BETA)[n:] * (RS_ROLLOFF * np.sinc(RS_ROLLOFF * np.linspace(0, RS_ZEROS, n + 1)))
+
+
+def resample_filter(sr_orig, sr_new):
+    """resampy 0.2.2's kaiser_best table as resample_f receives it for ratio = sr_new / sr_orig -> (win_delta float64
+    [32769, 2] = {win, delta}, step).  win = kaiser(2n+1, beta)[n:] * rolloff * sinc(rolloff * linspace(0, 64, n+1)),
+    n = 512*64, scaled by ratio when ratio < 1; delta[:-1] = diff(win), delta[-1] = 0; step = int(min(1, ratio) * 512).
+    Restated from the published algorithm: parity with a resampy build is not pinned."""
+    return _resample_filter(float(sr_new) / sr_orig)
+
+
+@functools.lru_cache(maxsize=None)
+def _resample_filter(ratio):
+    win = _kaiser_best().copy()
+    if ratio < 1:
+        win *= ratio
+    wd = np.zeros((len(win), 2))
+    wd[:, 0] = win
+    wd[:-1, 1] = np.diff(win)
+    wd.flags.writeable = False
+    return wd, int(min(1.0, ratio) * RS_TABLE)
+
+
+def resample_register(ratio, n):
+    """resample_f's time register for the first n outputs: treg[0] = 0, treg[t] = treg[t-1] + 1/ratio in float64, summed
+    in order (np.cumsum is that recurrence).  Not t/ratio: the kernels reproduce the truncations of the running sum."""
+    treg = np.zeros(n)
+    np.cumsum(np.full(n - 1, 1.0 / ratio), out=treg[1:])
+    return treg
+
+
+_rs_dev = {}
+
+
+def _resample_on(ratio, n, device):
+    """the table and a time register of at least n entries on `device`, cached per ratio; the register grows (its
+    prefix does not change) when a longer utterance arrives"""
+    key = (str(device), ratio)
+    wd, treg = _rs_dev.get(key, (None, None))
+    if wd is None:
+        wd = torch.from_numpy(_resample_filter(ratio)[0].copy()).to(device)
+    if treg is None or treg.numel() < n:
+        treg = torch.from_numpy(resample_register(ratio, n)).to(device)
+    _rs_dev[key] = (wd, treg)
+    return wd, treg
+
+
+def _upload(waves, device):
+    cuda = torch.device(device).type == "cuda"
+    y = torch.from_numpy(np.concatenate(waves).astype(np.float32, copy=False) if len(waves) else np.zeros(0, np.float32))
+    return (y.pin_memory() if cuda else y).to(device, non_blocking=True)
+
+
+def _resample_device(waves, rates, sr, K, device):
+    """the chunk on `device`, packed end to end in order with every utterance at `sr` -> (y, lengths int64).  One
+    resample launch per source rate; an utterance already at `sr` is copied unchanged."""
+    lens = np.array([len(w) for w in waves], dtype=np.int64)
+    groups = {}
+    for b, q in enumerate(rates):
+        if int(q) != sr:
+            groups.setdefault(int(q), []).append(b)
+    sizes = {b: resample_lengths(int(lens[b]), q, sr, f"utterance {b}") for q, idx in groups.items() for b in idx}
+    same = [b for b in range(len(waves)) if b not in sizes]
+    parts = [None] * len(waves)
+    if same:
+        y = _upload([waves[b] for b in same], device)
+        off = np.concatenate([[0], np.cumsum(lens[same])])
+        for j, b in enumerate(same):
+            parts[b] = y[off[j]:off[j + 1]]
+    for q, idx in groups.items():
+        ratio = float(sr) / q
+        n_out = max(sizes[b][0] for b in idx)
+        in_off = np.concatenate([[0], np.cumsum(lens[idx])]).astype(np.int64)
+        out_off = np.concatenate([[0], np.cumsum([sizes[b][1] for b in idx])]).astype(np.int64)
+        out = torch.empty(int(out_off[-1]), dtype=torch.float32, device=device)
+        wd, treg = _resample_on(ratio, n_out, device)
+        K.resample(out, _upload([waves[b] for b in idx], device), torch.from_numpy(in_off).to(device),
+                   torch.from_numpy(out_off).to(device), wd, _resample_filter(ratio)[1], ratio, treg[:n_out])
+        for j, b in enumerate(idx):
+            parts[b] = out[out_off[j]:out_off[j + 1]]
+            lens[b] = sizes[b][1]
+    return torch.cat(parts) if parts else torch.zeros(0, dtype=torch.float32, device=device), lens
+
+
+def resample_batch(waves, rates, sr, K=None, device="cuda"):
+    """librosa.resample(w, rates[b], sr, res_type='kaiser_best') (librosa 0.6 over resampy 0.2.2, as librosa.load(f,
+    sr=sr) applies it; audio.py:39) for each mono float32 waveform -> list of float32 numpy arrays of ceil(n*sr/rate)
+    samples.  A waveform already at `sr` is returned unchanged.  The arithmetic is resampy's loop, bit for bit, as restated
+    in resample_filter / resample_register (tests/resample_oracle.py); parity with resampy itself is not pinned."""
+    y, lens = _resample_device(waves, rates, sr, K or _K(), device)
+    y = y.cpu().numpy()
+    off = np.concatenate([[0], np.cumsum(lens)])
+    return [y[off[b]:off[b + 1]].copy() for b in range(len(waves))]
 
 
 def mel_basis(sr=MEL_SR, n_mels=N_MELS):
@@ -113,23 +236,30 @@ def _mel_on(device):
     return _mel_dev[key]
 
 
-def process_audio_batch(waves, r, K=None, device="cuda", out_dtype=torch.float16):
+def process_audio_batch(waves, r, K=None, device="cuda", out_dtype=torch.float16, rates=None, sr=None):
     """The reference's process_audio (audio.py:38-65) for a chunk of mono float32 waveforms (numpy, each at least
     1025 samples): trim silence, drop an utterance longer than maximum_audio_length after trimming, zero-pad, pre-emphasise,
     STFT, mel, log, reshape_frames(forward=True).  Returns (mel [n, T, 80 r], stft [n, T, 1025 r], keep [N] bool) with
-    the n = keep.sum() kept utterances in order, T = feature_frames_per_utterance(r); the arrays are on `device`."""
+    the n = keep.sum() kept utterances in order, T = feature_frames_per_utterance(r); the arrays are on `device`.
+    rates: the waveforms' sample rates; each one not at `sr` is first resampled to `sr` on the device as librosa.load does
+    (resample_batch), and the 1025-sample minimum applies to the result."""
     K = K or _K()
     T = feature_frames_per_utterance(r)
-    lens = np.array([len(w) for w in waves], dtype=np.int64)
+    y = None
+    if rates is not None and any(int(q) != sr for q in rates):
+        if sr is None:
+            raise ValueError("process_audio_batch: rates given without the target rate sr")
+        y, lens = _resample_device(waves, rates, sr, K, device)
+    else:
+        lens = np.array([len(w) for w in waves], dtype=np.int64)
     short = np.flatnonzero(lens < MIN_SAMPLES)
     if short.size:
         raise ValueError(f"utterance {int(short[0])} has {int(lens[short[0]])} samples; at least {MIN_SAMPLES} are needed")
     N = len(waves)
     offsets = np.zeros(N + 1, dtype=np.int64)
     np.cumsum(lens, out=offsets[1:])
-    cuda = torch.device(device).type == "cuda"
-    y = torch.from_numpy(np.concatenate(waves).astype(np.float32, copy=False) if N else np.zeros(0, np.float32))
-    y = (y.pin_memory() if cuda else y).to(device, non_blocking=True)
+    if y is None:
+        y = _upload(waves, device)
     bounds = torch.empty((N, 2), dtype=torch.int32, device=device)
     K.trim_bounds(bounds, y, torch.from_numpy(offsets).to(device), TRIM_FRAME, TRIM_HOP, TRIM_TOP_DB)
     b = bounds.cpu().numpy().astype(np.int64)

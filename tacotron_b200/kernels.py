@@ -445,6 +445,19 @@ def feature_spec(stft_out, mel_out, X, basis, lo, hi, r):
                                       _st()), "taco_feature_spec")
 
 
+def resample(out, y, in_off, out_off, win_delta, step, ratio, treg):
+    """out fp32 = librosa's kaiser_best resampling of each y[in_off[b]:in_off[b+1]] by one ratio into
+    out[out_off[b]:out_off[b+1]] (ceil(n_in*ratio) samples, zeros after int(n_in*ratio)).  win_delta float64 [nwin, 2],
+    treg float64 [>= the longest int(n_in*ratio)]: audio.resample_filter / audio.resample_register."""
+    B = in_off.numel() - 1
+    _cuda_c(out, torch.float32, "resample out"); _cuda_c(y, torch.float32, "resample y")
+    _cuda_c(in_off, torch.int64, "resample in_off"); _cuda_c(out_off, torch.int64, "resample out_off")
+    _cuda_c(win_delta, torch.float64, "resample win_delta"); _cuda_c(treg, torch.float64, "resample treg")
+    assert out_off.shape == (B + 1,) and win_delta.dim() == 2 and win_delta.shape[1] == 2 and treg.dim() == 1
+    L.check(L.lib().taco_resample(_p(out), _p(y), _p(in_off), _p(out_off), B, _p(win_delta), win_delta.shape[0], int(step),
+                                  float(ratio), _p(treg), treg.numel(), _st()), "taco_resample")
+
+
 _ss_ws = {}
 
 

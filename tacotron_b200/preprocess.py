@@ -3,7 +3,7 @@ and ``meta.pkl`` that ``tacotron_b200.data_input.load_from_npy`` reads.  Host mi
 (same names: ``prepare_arctic / prepare_nancy / prepare_vctk``, ``process_char``, ``pad_to_dense``, ``save_to_npy``,
 ``save_vocab``, ``preprocess``) with the feature extraction on the GPU (``audio.process_audio_batch``).
 
-    python -m tacotron_b200.preprocess {arctic,nancy,vctk} [--data-dir data/] [-r 2]
+    python -m tacotron_b200.preprocess {arctic,nancy,vctk} [--data-dir data/] [-r 2] [--resample]
 
 Kept from the reference: the file layouts of the three corpora (preprocess.py:41-117); characters enter the vocabulary in
 first-seen order with <pad> = 0, including the characters of utterances that are later dropped (:186-189); texts are
@@ -15,8 +15,11 @@ Deliberate deviations:
     speakers and utterances whenever one is dropped.
   * meta['sr'] is the rate actually used.  The reference always writes 16000 (save_vocab is called without sr, :208).
   * r = 4 (and any r outside 1-6) is rejected: the reference crashes on it (see audio.feature_frames_per_utterance).
-  * a file whose rate differs from the corpus rate is an error naming the file (resampling is not implemented), and so
-    is a file shorter than 1025 samples (too short for the STFT's reflect padding).
+  * a file whose rate differs from the corpus rate is an error naming the file unless --resample is given; with it, such
+    a file is resampled on the GPU as the reference's librosa.load(f, sr=sr) does (audio.resample_batch: librosa 0.6's
+    kaiser_best over resampy 0.2.2's loop, restated; parity with resampy itself is not pinned).  A file too short to
+    give one resampled sample is an error naming it, and so is a file shorter than 1025 samples at the corpus rate (too
+    short for the STFT's reflect padding).
 
 Work is done in chunks.  A reader thread decodes the WAVs of the next chunk while the GPU works on the current one; the
 float16 results are copied to pinned host buffers asynchronously and written to ``np.lib.format.open_memmap`` files while
@@ -67,7 +70,8 @@ def prepare_nancy(data_dir):
 
 def prepare_vctk(data_dir):
     """preprocess.py:81-117: speakers from the ID column of vctk/speaker-info.txt (ids in file order), prompts from
-    vctk/txt/p<ID>/*.txt, wavs in vctk/wav48/p<ID>/ -- which must already be at 24 kHz (no resampling here)."""
+    vctk/txt/p<ID>/*.txt, wavs in vctk/wav48/p<ID>/: the original 48 kHz files with --resample (preprocess(...,
+    resample=True)), otherwise files already converted to 24 kHz."""
     root = os.path.join(data_dir, "vctk")
     with open(os.path.join(root, "speaker-info.txt")) as f:
         header = f.readline().split()
@@ -134,17 +138,27 @@ def _shrink_npy(path, rows):
         f.truncate(10 + hlen + rows * int(np.prod(shape[1:])) * np.dtype(d["descr"]).itemsize)
 
 
-def _reader(files, sr, chunk, q):
+def _reader(files, sr, chunk, q, resample=False):
+    """queues (i, chunk of samples), or with `resample` (i, chunk of (samples, rate))"""
     try:
         for i in range(0, len(files), chunk):
-            q.put((i, [audio.load_wav(f, sr) for f in files[i:i + chunk]]))
+            if not resample:
+                q.put((i, [audio.load_wav(f, sr) for f in files[i:i + chunk]]))
+                continue
+            items = [audio.read_wav(f) for f in files[i:i + chunk]]
+            for f, (x, rate) in zip(files[i:i + chunk], items):
+                if rate != sr:
+                    audio.resample_lengths(len(x), rate, sr, f)          # raises, naming the file, if nothing is left
+            q.put((i, items))
         q.put(None)
     except BaseException as e:                                    # re-raised in the consumer
         q.put(e)
 
 
-def preprocess(data, out_dir, r=2, sr=16000, chunk=CHUNK, K=None, device="cuda", log=print):
-    """preprocess.py:168-208: features of every listed utterance into <out_dir>; returns the number kept"""
+def preprocess(data, out_dir, r=2, sr=16000, chunk=CHUNK, K=None, device="cuda", log=print, resample=False):
+    """preprocess.py:168-208: features of every listed utterance into <out_dir>; returns the number kept.  resample: a
+    file at another rate is resampled to `sr` on the device (librosa.load's kaiser_best, audio.resample_batch) instead
+    of being an error; meta['sr'] is `sr` either way."""
     os.makedirs(out_dir, exist_ok=True)
     T = audio.feature_frames_per_utterance(r)
     vocab, ivocab = {"<pad>": 0}, {0: "<pad>"}
@@ -156,7 +170,7 @@ def preprocess(data, out_dir, r=2, sr=16000, chunk=CHUNK, K=None, device="cuda",
     stfts = np.lib.format.open_memmap(os.path.join(out_dir, "stfts.npy"), mode="w+", dtype=np.float16, shape=(N, T, audio.F_BINS * r))
     cuda = torch.device(device).type == "cuda"
     q = queue.Queue(maxsize=2)
-    th = threading.Thread(target=_reader, args=(files, sr, chunk, q), daemon=True)
+    th = threading.Thread(target=_reader, args=(files, sr, chunk, q, resample), daemon=True)
     th.start()
     kept = []
     count = 0
@@ -179,8 +193,11 @@ def preprocess(data, out_dir, r=2, sr=16000, chunk=CHUNK, K=None, device="cuda",
         if item is None:
             break
         i, waves = item
+        rates = None
+        if resample:
+            waves, rates = [x for x, _ in waves], [rate for _, rate in waves]
         try:
-            mel, stft, keep = audio.process_audio_batch(waves, r, K=K, device=device)
+            mel, stft, keep = audio.process_audio_batch(waves, r, K=K, device=device, rates=rates, sr=sr)
         except ValueError as e:
             raise ValueError(f"chunk starting at {files[i]}: {e}") from None
         kept.extend(i + np.flatnonzero(keep))
@@ -218,11 +235,14 @@ def main(argv=None):
     parser.add_argument("dataset", choices=sorted(prepare_functions))
     parser.add_argument("--data-dir", default="data/")
     parser.add_argument("-r", type=int, default=2, help="decoder frames per step the arrays are laid out for")
+    parser.add_argument("--resample", action="store_true",
+                        help="resample files at other rates to the corpus rate on the GPU (librosa.load's kaiser_best), "
+                             "e.g. VCTK's 48 kHz originals, instead of rejecting them")
     args = parser.parse_args(argv)
     audio.feature_frames_per_utterance(args.r)
     data = prepare_functions[args.dataset](args.data_dir)
     sr = SR[args.dataset]
-    n = preprocess(data, os.path.join(args.data_dir, args.dataset), r=args.r, sr=sr)
+    n = preprocess(data, os.path.join(args.data_dir, args.dataset), r=args.r, sr=sr, resample=args.resample)
     print(f"{n} of {len(data['prompts'])} utterances written to {os.path.join(args.data_dir, args.dataset)}")
 
 
