@@ -365,6 +365,20 @@ int taco_feature_spec(void* stft_out, void* mel_out, int out_f16, const float* X
 int taco_resample(float* out, const float* in, const int64_t* in_off, const int64_t* out_off, int B, const double* win_delta,
                   int nwin, int step, double ratio, const double* treg, int64_t treg_len, void* stream);
 
+/* ==========================================================================================
+ * Training summaries: tf.summary.histogram (models/tacotron.py:129,139,152) = TF 1.2's HistogramSummaryOp /
+ * histogram::Histogram::Add over x [n] fp32 (16-byte aligned), reduced on the device.  limits [nlim] float64 = TF's default
+ * bucket table (nlim = 1551: -DBL_MAX, the mirrored negatives, 0.0 at 775, the positives 1e-12 * 1.1^k by repeated
+ * multiplication while < 1e20, DBL_MAX).  A finite value x goes to counts[upper_bound(limits, (double)x) - limits];
+ * stats = {min, max, sum, sum of squares} of the widened finite values (min = DBL_MAX, max = -DBL_MAX when there are none);
+ * NaN / Inf elements are counted in nonfinite[0], not binned.  Counts, min and max exact; sum and sum of squares from a
+ * fixed grid and reduction order (bit-identical from run to run).  workspace: taco_histogram_workspace_bytes(), 16-byte
+ * aligned.  Semantics: tests/mirror_kernels_summary.py.
+ * ========================================================================================== */
+size_t taco_histogram_workspace_bytes(void);
+int    taco_histogram(const float* x, int64_t n, const double* limits, int nlim, void* workspace, int64_t* counts,
+                      double* stats, int64_t* nonfinite, void* stream);
+
 int taco_sumsq(const float* x, int64_t n, float* partial_ws, float* out, void* stream);
 int taco_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr_t, float b1, float b2, float eps,
                    float clip, const float* sumsq, void* stream);

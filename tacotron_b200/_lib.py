@@ -107,6 +107,8 @@ EXPORTS = [
     "taco_normalize_f16",
     # feature extraction (preprocessing)
     "taco_trim_bounds", "taco_feature_frames", "taco_feature_spec", "taco_resample",
+    # training summaries
+    "taco_histogram_workspace_bytes", "taco_histogram",
 ]
 
 
@@ -176,6 +178,8 @@ def lib():
     L.taco_feature_frames.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
     L.taco_feature_spec.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     L.taco_resample.argtypes = [vp, vp, vp, vp, i32, vp, i32, i32, C.c_double, vp, i64, vp]
+    L.taco_histogram_workspace_bytes.restype = C.c_size_t
+    L.taco_histogram.argtypes = [vp, i64, vp, i32, vp, vp, vp, vp, vp]
     for name in EXPORTS:                      # every declared symbol must resolve (AttributeError otherwise)
         getattr(L, name)
     _lib = L

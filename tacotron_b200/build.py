@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtaco_b200.so")
 SOURCES = ["api.cu", "gemm_simt.cu", "gemm_tc.cu", "gru.cu", "decoder.cu", "train.cu", "gru_bwd.cu", "decoder_bwd.cu", "audio.cu", "data.cu", "features.cu",
-           "resample.cu"]
+           "resample.cu", "summary.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

@@ -458,6 +458,25 @@ def resample(out, y, in_off, out_off, win_delta, step, ratio, treg):
                                   float(ratio), _p(treg), treg.numel(), _st()), "taco_resample")
 
 
+# ---- training summaries (tacotron_b200/summary.py) ----
+_hist_ws = {}
+
+
+def histogram(res, x, limits):
+    """TF 1.2's histogram of x (contiguous CUDA fp32, 16-byte aligned) into res int64 [nlim + 5]: res[:nlim] the bucket
+    counts (a finite value goes to upper_bound(limits, value)), res[nlim] the NaN / Inf count (not binned),
+    res[nlim+1:].view(float64) = {min, max, sum, sum of squares} of the finite values.  limits float64 [nlim] on the
+    device = summary.histogram_limits()."""
+    nlim = limits.numel()
+    _cuda_c(x, torch.float32, "histogram x"); _cuda_c(res, torch.int64, "histogram res"); _cuda_c(limits, torch.float64, "histogram limits")
+    assert res.shape == (nlim + 5,)
+    ws = _hist_ws.get(x.device)
+    if ws is None:
+        ws = _hist_ws[x.device] = torch.empty(L.lib().taco_histogram_workspace_bytes(), dtype=torch.uint8, device=x.device)
+    L.check(L.lib().taco_histogram(_p(x), x.numel(), _p(limits), nlim, _p(ws), _p(res), C.c_void_p(res.data_ptr() + 8 * (nlim + 1)),
+                                   C.c_void_p(res.data_ptr() + 8 * nlim), _st()), "taco_histogram")
+
+
 _ss_ws = {}
 
 

@@ -6,8 +6,9 @@
 Prompts come from stdin, one per line (test.py:77-78); they are encoded and padded to 140 characters exactly as
 ``data_input.load_prompts`` does (quirks included), run through ``Tacotron.inference`` in batches of at most 32, every
 output is de-normalised with the checkpoint's ``stft_mean`` / ``stft_std`` and inverted with the GPU Griffin-Lim
-(test.py:59-64).  Instead of TensorBoard summaries the waveform is written as ``log/<save_path>/test/<n>.wav`` and the
-alignment as ``<n>_attention.npy``.
+(test.py:59-64).  The waveform is written as ``log/<save_path>/test/<n>.wav`` and the alignment as
+``<n>_attention.npy``; with ``--summaries`` the reference's TensorBoard audio and image summaries go next to them
+(:33, :65-69; tacotron_b200/summary.py).
 """
 from __future__ import annotations
 
@@ -19,7 +20,9 @@ import numpy as np
 import torch
 
 
-def test(model_cls, config, prompts, log=print, speaker=0):
+def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None):
+    """summary_dir: also write each prompt's audio and attention image as TensorBoard summaries there, at step 0
+    (tacotron_b200/summary.py)"""
     from . import audio, checkpoint, data_input
     from .train import write_wav
     sr = 24000 if "blizzard" in config.data_path else 16000                              # test.py:15
@@ -55,23 +58,36 @@ def test(model_cls, config, prompts, log=print, speaker=0):
     std_d = torch.from_numpy(np.asarray(stft_std, dtype=np.float32)).cuda()
     out_dir = os.path.join("log", config.save_path, "test")                              # :33
     os.makedirs(out_dir, exist_ok=True)
+    writer = None
+    if summary_dir is not None:                                                          # :33
+        from . import summary
+        writer, scopes = summary.EventWriter(summary_dir), summary.NameScopes()
     n = 0
     waves = []
-    for inputs in data_input.load_prompts(prompts, ivocab):                              # :21-22, :50-56
-        if config.num_speakers > 1:
-            inputs["speaker"] = torch.full((inputs["text"].shape[0],), speaker, dtype=torch.int32, device=inputs["text"].device)
-        _, outputs = model.inference(inputs, train=False)
-        alignments = model.alignments
-        log("saving samples")
-        wav = audio.invert_spectrogram(outputs, config.r, stft_mean=mean_d, stft_std=std_d)     # :64, batched on the device
-        for b in range(outputs.shape[0]):                                                # :59-70
-            text = "".join(ivocab[int(w)] for w in inputs["text"][b].cpu().numpy())
-            write_wav(os.path.join(out_dir, f"{n}.wav"), wav[b].cpu().numpy(), sr)
-            np.save(os.path.join(out_dir, f"{n}_attention.npy"), alignments[b].cpu().numpy())
-            with open(os.path.join(out_dir, f"{n}.txt"), "w") as f:
-                f.write(text)
-            waves.append(wav[b])
-            n += 1
+    try:
+        for inputs in data_input.load_prompts(prompts, ivocab):                          # :21-22, :50-56
+            if config.num_speakers > 1:
+                inputs["speaker"] = torch.full((inputs["text"].shape[0],), speaker, dtype=torch.int32, device=inputs["text"].device)
+            _, outputs = model.inference(inputs, train=False)
+            alignments = model.alignments
+            log("saving samples")
+            wav = audio.invert_spectrogram(outputs, config.r, stft_mean=mean_d, stft_std=std_d)   # :64, batched on the device
+            for b in range(outputs.shape[0]):                                            # :59-70
+                text = "".join(ivocab[int(w)] for w in inputs["text"][b].cpu().numpy())
+                wave, alignment = wav[b].cpu().numpy(), alignments[b].cpu().numpy()
+                write_wav(os.path.join(out_dir, f"{n}.wav"), wave, sr)
+                np.save(os.path.join(out_dir, f"{n}_attention.npy"), alignment)
+                with open(os.path.join(out_dir, f"{n}.txt"), "w") as f:
+                    f.write(text)
+                if writer is not None:           # :65-69: audio(text) then image(text), name scopes of one graph
+                    tag = summary.clean_tag(text)
+                    writer.add(0, [summary.audio_value(scopes.unique(tag) + "/audio/0", wave, sr),
+                                   summary.image_value(scopes.unique(tag) + "/image/0", summary.attention_rgba(alignment))])
+                waves.append(wav[b])
+                n += 1
+    finally:
+        if writer is not None:
+            writer.close()
     return waves
 
 
@@ -79,6 +95,7 @@ def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", "--train-set", default="nancy")
     parser.add_argument("-s", "--speaker", type=int, default=0, help="speaker id of a multi-speaker model")
+    parser.add_argument("--summaries", action="store_true", help="write TensorBoard summaries to log/<save_path>/test")
     args = parser.parse_args(argv)
     prompts = [p for p in sys.stdin.readlines() if len(p) > 0]                           # test.py:77-78
     from .models.tacotron import Config, Tacotron
@@ -86,7 +103,8 @@ def main(argv=None):
     config.data_path = "data/%s/" % args.train_set                                       # :83
     config.save_path = args.train_set + "/tacotron"                                      # :84
     print("Building Tacotron")
-    test(Tacotron, config, prompts, speaker=args.speaker)
+    summary_dir = os.path.join("log", config.save_path, "test") if args.summaries else None      # test.py:33
+    test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir)
 
 
 if __name__ == "__main__":

@@ -6,8 +6,9 @@
 Kept from the reference: data_path / save_path conventions (:107-113), meta.pkl supplies r and the vocabulary (:19-22),
 lr fed per step starting at ``init_lr`` and multiplied by ``annealing_rate`` every 1000 steps (:60-61, :79-80), the
 explosion guard ``loss > 1e8 and global_step > 500`` (:75-77), a checkpoint + an audio sample every SAVE_EVERY steps
-(:82-101; the sample is inverted with the GPU Griffin-Lim and written as .wav next to the checkpoint instead of a
-TensorBoard audio summary, the alignment as .npy instead of a matplotlib image).  Data parallel ranks draw disjoint
+(:82-101; the sample is inverted with the GPU Griffin-Lim and written as .wav next to the checkpoint, the alignment as
+.npy).  With ``--summaries`` the reference's TensorBoard summaries are written as well (:41, :64-75, :92-103;
+tacotron_b200/summary.py).  Data parallel ranks draw disjoint
 batches of 32 and all-reduce the flat gradient bucket inside ``model.train_step`` (tacotron_b200/optim.py).
 """
 from __future__ import annotations
@@ -30,7 +31,10 @@ def write_wav(path, wave, sr):
     wavfile.write(path, sr, (w / peak * 0.95 * 32767).astype(np.int16))
 
 
-def train(model_cls, config, num_steps=1000000, log=print, save_every=SAVE_EVERY):
+def train(model_cls, config, num_steps=1000000, log=print, save_every=SAVE_EVERY, summary_dir=None, summary_every=1):
+    """summary_dir: write TensorBoard summaries there (tacotron_b200/summary.py): the losses, the global gradient norm and
+    the histograms of the pre-net output, seq2seq_output and output every `summary_every` steps, the two clips and the
+    attention image at every save step.  The histograms are rank 0's batch."""
     from . import audio, checkpoint, data_input
     from .utils import dist as D
     world, rank, local = D.world()
@@ -61,30 +65,51 @@ def train(model_cls, config, num_steps=1000000, log=print, save_every=SAVE_EVERY
     std_d = torch.from_numpy(np.asarray(stft_std, dtype=np.float32)).cuda()
     lr = model.config.init_lr                                                            # :60
     annealing_rate = model.config.annealing_rate                                         # :61
-    for _ in range(num_steps):                                                           # :63
-        inputs = next(batches)
-        loss_t = train_op(inputs, lr).reshape(1).clone()                                 # :64-73
-        if world > 1:                      # every rank must take the same branch below (a rank that leaves alone hangs the
-            torch.distributed.all_reduce(loss_t)   # next gradient all-reduce): the guard and the log use the global loss
-        loss = float(loss_t)                                                             # the only host sync of a step
-        global_step = model.global_step
-        if rank == 0 and global_step % 100 == 0:
-            log(f"step {global_step} loss {loss:.1f} lr {lr:.3g} grad-norm {float(model.grad_sumsq.sqrt()):.1f}")
-        if loss > 1e8 and global_step > 500:                                             # :75-77 detect gradient explosion
-            log("loss exploded")
-            break
-        if global_step % 1000 == 0:                                                      # :79-80
-            lr *= annealing_rate
-        if global_step % save_every == 0 and global_step != 0 and rank == 0:             # :82
-            log("saving weights")
-            fn = checkpoint.save(model, weights_dir, stft_mean, stft_std)                # :85-88
-            log("saving sample")                                                         # :90-101
-            ideal = audio.invert_spectrogram(inputs["stft"][0], config.r, stft_mean=mean_d, stft_std=std_d)
-            sample = audio.invert_spectrogram(model.output[0], config.r, stft_mean=mean_d, stft_std=std_d)
-            base = fn[:-4]
-            write_wav(base + "_ideal.wav", ideal.cpu().numpy(), sr)
-            write_wav(base + "_sample.wav", sample.cpu().numpy(), sr)
-            np.save(base + "_attention.npy", model.alignments[0].cpu().numpy())
+    # summaries (train.py:41,64-75): rank 0 writes; every rank takes part in the one all-reduce of the three losses
+    summaries = None
+    if summary_dir is not None and rank == 0:
+        from . import summary
+        summaries = summary.TrainSummaries(summary_dir, torch.device("cuda", local), log)
+    try:
+        for _ in range(num_steps):                                                       # :63
+            inputs = next(batches)
+            loss_t = train_op(inputs, lr).reshape(1).clone()                             # :64-73
+            if summary_dir is not None:
+                loss_t = torch.stack([model.loss, model.seq2seq_loss, model.output_loss])
+            if world > 1:                  # every rank must take the same branch below (a rank that leaves alone hangs the
+                torch.distributed.all_reduce(loss_t)   # next gradient all-reduce): the guard and the log use the global loss
+            global_step = model.global_step
+            if summaries is not None:
+                if global_step % summary_every == 0:
+                    summaries.enqueue(global_step, (model.saved["enc/prenet/l2"], model.seq2seq_output, model.output), loss_t,
+                                      model.grad_sumsq)
+                summaries.write_pending()          # the previous step's records, encoded while the GPU runs this step
+            loss = float(loss_t[0])                                                      # the only host sync of a step
+            if summaries is not None:
+                summaries.collect()
+            if rank == 0 and global_step % 100 == 0:
+                log(f"step {global_step} loss {loss:.1f} lr {lr:.3g} grad-norm {float(model.grad_sumsq.sqrt()):.1f}")
+            if loss > 1e8 and global_step > 500:                                         # :75-77 detect gradient explosion
+                log("loss exploded")
+                break
+            if global_step % 1000 == 0:                                                  # :79-80
+                lr *= annealing_rate
+            if global_step % save_every == 0 and global_step != 0 and rank == 0:         # :82
+                log("saving weights")
+                fn = checkpoint.save(model, weights_dir, stft_mean, stft_std)            # :85-88
+                log("saving sample")                                                     # :90-101
+                ideal = audio.invert_spectrogram(inputs["stft"][0], config.r, stft_mean=mean_d, stft_std=std_d).cpu().numpy()
+                sample = audio.invert_spectrogram(model.output[0], config.r, stft_mean=mean_d, stft_std=std_d).cpu().numpy()
+                alignment = model.alignments[0].cpu().numpy()
+                base = fn[:-4]
+                write_wav(base + "_ideal.wav", ideal, sr)
+                write_wav(base + "_sample.wav", sample, sr)
+                np.save(base + "_attention.npy", alignment)
+                if summaries is not None:
+                    summaries.save_step(global_step, ideal, sample, alignment, sr)
+    finally:
+        if summaries is not None:
+            summaries.close()
     return model
 
 
@@ -94,6 +119,8 @@ def main(argv=None):
     parser.add_argument("-d", "--debug", type=bool, default=False)
     parser.add_argument("-r", "--restore", type=bool, default=False)
     parser.add_argument("--steps", type=int, default=1000000)
+    parser.add_argument("--summaries", action="store_true", help="write TensorBoard summaries to log/<save_path>/train")
+    parser.add_argument("--summary-every", type=int, default=1, help="steps between two per-step summaries")
     args = parser.parse_args(argv)
     from .models.tacotron import Config, Tacotron
     config = Config()
@@ -101,7 +128,8 @@ def main(argv=None):
     config.restore = args.restore
     config.save_path = "debug" if args.debug else "%s/tacotron" % args.train_set         # :110-113
     print("Building Tacotron")
-    train(Tacotron, config, num_steps=args.steps)
+    summary_dir = os.path.join("log", config.save_path, "train") if args.summaries else None     # train.py:41
+    train(Tacotron, config, num_steps=args.steps, summary_dir=summary_dir, summary_every=args.summary_every)
 
 
 if __name__ == "__main__":
