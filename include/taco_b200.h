@@ -139,9 +139,10 @@ int taco_bigru_fwd_h0(const float* xp, const float* Wg_h_fw, const float* Wc_h_f
  * Decoder: tacotron.py:46-105 create_decoder + :136-138 dynamic_decode, i.e. per step
  *   pre_net(last frame) ++ attention -> InputProjection -> 3x GRUCell(256) -> Residual ->
  *   OutputProjection(80r) -> BahdanauAttention(query = cell output) -> attention layer.
- * The whole T-step loop runs in ONE persistent kernel: 128 co-resident CTAs (one per SM), activations exchanged as
- * {value, step tag} words through L2, weights in shared memory and L2 (csrc/decoder.cu).  Tx in [1,256], any
- * width (the four attention quarters are ragged when Tx % 4 != 0); B <= 32 per launch; 80 r <= 512.
+ * The whole T-step loop runs in ONE persistent kernel: 32 co-resident CTAs (one per SM) per row group of 8 utterances,
+ * min(4, CTA budget / 32) row groups per launch (128 CTAs when the device holds them), activations exchanged as
+ * {value, step tag} words through L2, weights in shared memory and L2 (csrc/decoder.cu).  Tx in [1,256], any width (the
+ * four attention quarters are ragged when Tx % 4 != 0); B <= 8 * row groups (<= 32) per launch; 80 r <= 512.
  * ------------------------------------------------------------------------------------------ */
 typedef struct taco_decoder_weights {   /* all TF layout, device pointers */
     const float *pre_W1, *pre_b1, *pre_W2, *pre_b2;      /* [80][256],[256],[256][128],[128]   */
@@ -176,9 +177,17 @@ typedef struct taco_decoder_args {
     uint64_t*      step_ns;      /* [T] device buffer: %globaltimer at the start of each step, or NULL */
     float*         h_save;       /* [3][T][B][256] the three GRU state sequences (training: input of
                                     taco_decoder_bwd's batched recomputation), or NULL          */
+    int32_t        row0;         /* the [T][B]-major tensors (sample_mask, keep1, keep2, h_save) have   */
+    int32_t        row_stride;   /* row_stride rows per step, this launch's row b is row0 + b (a batch
+                                    decoded in several launches); row_stride = 0: B rows, row0 = 0   */
+    int32_t        max_ctas;     /* CTA budget (>= 32), 0 = what the device holds (taco_decoder_capacity) */
 } taco_decoder_args;
 
 int taco_decoder_fwd(const taco_decoder_args* a, void* stream);
+/* co-resident CTAs of the forward (taco_decoder_fwd) and backward (taco_decoder_bwd) decoder kernels on the current
+ * device (either pointer may be NULL).  The forward runs 32 CTAs per row group of 8 utterances, the backward at least 32
+ * and at most 128 CTAs.                                                                                              */
+int taco_decoder_capacity(int* fwd_ctas, int* bwd_ctas);
 
 /* tacotron.py:156-160: partial[0] = sum|a-b| over n elements (deterministic two-stage).       */
 int taco_l1_loss_fwd(const float* a, const float* b, int64_t n, float* partial_ws, float* out, void* stream);
@@ -292,6 +301,8 @@ typedef struct taco_decoder_bwd_args {
     float *DSCORE;                        /* out: [B][T][Tx]                                            */
     float *DCTX, *DG[3], *DC[3], *DZ, *DPN2, *DPN1, *DX;
     float *workspace;                     /* taco_decoder_bwd_workspace_bytes                           */
+    int32_t max_ctas;                     /* CTA budget (>= 32), 0 = what the device holds; the kernel runs on
+                                             min(budget, capacity, 128) CTAs                                */
 } taco_decoder_bwd_args;
 size_t taco_decoder_bwd_workspace_bytes(void);
 int    taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream);

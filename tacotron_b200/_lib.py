@@ -55,6 +55,7 @@ class DecoderArgs(C.Structure):
         ("B", C.c_int32), ("Tx", C.c_int32), ("T", C.c_int32), ("r", C.c_int32),
         ("y", C.c_void_p), ("align", C.c_void_p), ("workspace", C.c_void_p), ("step_ns", C.c_void_p),
         ("h_save", C.c_void_p),
+        ("row0", C.c_int32), ("row_stride", C.c_int32), ("max_ctas", C.c_int32),
     ]
 
 
@@ -80,7 +81,7 @@ class DecoderBwdArgs(C.Structure):
         ("PQ", C.c_void_p), ("PN1", C.c_void_p), ("PN2", C.c_void_p), ("sel", C.c_void_p),
         ("DATT", C.c_void_p), ("DY", C.c_void_p), ("DPQ", C.c_void_p), ("DSCORE", C.c_void_p),
         ("DCTX", C.c_void_p), ("DG", C.c_void_p * 3), ("DC", C.c_void_p * 3), ("DZ", C.c_void_p), ("DPN2", C.c_void_p),
-        ("DPN1", C.c_void_p), ("DX", C.c_void_p), ("workspace", C.c_void_p),
+        ("DPN1", C.c_void_p), ("DX", C.c_void_p), ("workspace", C.c_void_p), ("max_ctas", C.c_int32),
     ]
 
 
@@ -95,6 +96,7 @@ EXPORTS = [
     "taco_last_error", "taco_version", "taco_device_info", "taco_linear_fwd", "taco_pack_weight", "taco_pack_weight_x3",
     "taco_maxpool_fwd", "taco_gather_rows", "taco_mask_rows", "taco_bigru_fwd", "taco_bigru_fwd_h0",
     "taco_decoder_packed_bytes", "taco_decoder_workspace_bytes", "taco_decoder_pack", "taco_decoder_fwd",
+    "taco_decoder_capacity",
     "taco_l1_loss_fwd", "taco_l1_partial_count", "taco_launch_count",
     # training path
     "taco_gemm", "taco_set_gemm_impl", "taco_conv_dw", "taco_colsum", "taco_colsum_seg", "taco_bias_act", "taco_mul_shift", "taco_epi_bwd", "taco_epi_fwd_keep", "taco_bn_param_grad",
@@ -141,6 +143,7 @@ def lib():
     L.taco_decoder_workspace_bytes.restype = C.c_size_t
     L.taco_decoder_pack.argtypes = [C.POINTER(DecoderWeights), C.c_int, C.c_void_p, C.c_void_p]
     L.taco_decoder_fwd.argtypes = [C.POINTER(DecoderArgs), C.c_void_p]
+    L.taco_decoder_capacity.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.taco_l1_loss_fwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     L.taco_l1_partial_count.restype = C.c_int
     L.taco_launch_count.restype = C.c_ulonglong

@@ -48,7 +48,8 @@
 //     tanh(k+q) = 1 - 2/(e^{2k} e^{2q} + 1) with e^{2k} precomputed once and e^{2q} once per step: one MUFU per
 //     element instead of two.
 //
-// Unchanged from v3: grid = 128 co-resident CTAs x 256 threads, CTA (rg, cs) owns utterance rows 8rg..8rg+7 and the
+// Unchanged from v3: grid = 32 co-resident CTAs per row group of 8 utterances (128 = 4 row groups when the device holds
+// them), CTA (rg, cs) owns utterance rows 8rg..8rg+7 and the
 // cs-th of 32 column slices of every dense stage; NO grid barrier: every exchanged activation is a 64-bit word
 // {fp32 value, step tag} written with one st.b64 and read with polling 128-bit loads; 3xTF32 error-compensated
 // tensor-core products (fp32-grade); GRU gate columns permuted so r,u of a hidden unit live in one CTA.
@@ -323,13 +324,15 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     const int g = lane >> 2, tg = lane & 3;            // MMA fragment coordinates
     const int cta = blockIdx.x;
     // dense stages: row group = the 32 consecutive CTAs that also run the attention of those 8 utterances, so the four
-    // row groups are four INDEPENDENT 32-CTA machines on (mostly) neighbouring SMs: no exchange crosses a group
+    // row groups are INDEPENDENT 32-CTA machines on (mostly) neighbouring SMs: no exchange crosses a group.  A launch runs
+    // gridDim.x / 32 of them (as many as the CTA budget allows, up to 4) over a prefix of the workspace.
     const int rg = cta >> 5, cs = cta & 31;
     const int arow = cta >> 2;                          // attention: utterance, quarter aq of its memory
     const uint32_t aq = (uint32_t)(cta & 3);
     const taco_decoder_args& A = P.a;
     uint64_t* ws = reinterpret_cast<uint64_t*>(A.workspace);
     const int B = A.B, T = A.T, OUT = P.OUT, Tq = P.Tq, Tx = A.Tx, NCY = P.NCY;
+    const int RS = A.row_stride, R0 = A.row0;          // [T][B]-major tensors: row r of this launch is full-batch row R0 + r
     const int row0 = rg * RPG;
     const int myrow = row0 + g;                        // the utterance row this lane's B fragments belong to
     const int lane_w = g * 8 + 2 * tg;                  // this lane's word offset inside a k-tile block
@@ -622,7 +625,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
         const int widx = warp - 8;
         bool from_y = (tb > 0);
         if (A.mode == TACO_DEC_TEACHER) from_y = false;
-        else if (A.mode == TACO_DEC_SCHED) from_y = (tb > 0) && (myrow < B) && (A.sample_mask[(int64_t)(tb - 1) * B + myrow] != 0);
+        else if (A.mode == TACO_DEC_SCHED) from_y = (tb > 0) && (myrow < B) && (A.sample_mask[(int64_t)(tb - 1) * RS + R0 + myrow] != 0);
         const uint64_t* p0 = ws + P.buf[from_y ? B_P1Y : B_P1M] + (int64_t)rg * 2048 + widx * 64 + lane_w;
         const uint32_t w1 = seg_word(P.seg[SG_P2], cs);
         issue_loads<4>(v, p0, 32, widx, 8, 0);
@@ -642,7 +645,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
 #pragma unroll
             for (int w = 0; w < 8; ++w) pv += part2_s[w * 64 + pi];
             pv = fmaxf(pv, 0.f);
-            if (A.keep2 && row < B && tb < T) pv = A.keep2[((int64_t)tb * B + row) * 128 + col] ? pv * A.keep_scale : 0.f;
+            if (A.keep2 && row < B && tb < T) pv = A.keep2[((int64_t)tb * RS + R0 + row) * 128 + col] ? pv * A.keep_scale : 0.f;
             ll_store(ws + otab[O_P2] + brow * 8 + perm8(4 * (cs & 1) + wcol), pv, tag);
         }
         named_bar(2, 256);                               // part2_s may be rewritten
@@ -707,14 +710,14 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
                     h_loc[gi * 64 + e_loc] = hn;
                     ll_store(ws + otab[O_H0 + gi] + e_word, hn, tag);
                     if (gi == 2) ll_store(ws + otab[O_S] + e_word, z_loc[e_loc] + hn, tag);
-                    if (A.h_save && e_row < B) A.h_save[(((int64_t)gi * T + t) * B + e_row) * U + 8 * cs + e_wc] = hn;   // training: BPTT input
+                    if (A.h_save && e_row < B) A.h_save[(((int64_t)gi * T + t) * RS + R0 + e_row) * U + 8 * cs + e_wc] = hn;   // training: BPTT input
                 }
                 break;
             case ST_PM:
                 if (tid < 64) {                              // here t = tb, the step the pre-net output belongs to
                     const int col = 8 * cs + e_wc;
                     float pv = fmaxf(sum16(part, e_pidx) + bias_s[BR_PM * 16 + e_wc], 0.f);
-                    if (A.keep1 && e_row < B && t < T) pv = A.keep1[((int64_t)t * B + e_row) * 256 + col] ? pv * A.keep_scale : 0.f;
+                    if (A.keep1 && e_row < B && t < T) pv = A.keep1[((int64_t)t * RS + R0 + e_row) * 256 + col] ? pv * A.keep_scale : 0.f;
                     ll_store(ws + otab[O_P1M] + e_word, pv, tag);
                 }
                 break;
@@ -729,7 +732,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
                 } else {                                     // p1(t+1) of free-running rows
                     const int col = 8 * cs + e_wc, tb = t + 1;
                     float pv = fmaxf(v0, 0.f);
-                    if (A.keep1 && e_row < B && tb < T) pv = A.keep1[((int64_t)tb * B + e_row) * 256 + col] ? pv * A.keep_scale : 0.f;
+                    if (A.keep1 && e_row < B && tb < T) pv = A.keep1[((int64_t)tb * RS + R0 + e_row) * 256 + col] ? pv * A.keep_scale : 0.f;
                     ll_store(ws + otab[O_P1Y] + e_word, pv, tag + 1);
                 }
             } break;
@@ -910,7 +913,37 @@ void build_ws_layout(int64_t* buf, int64_t* att, int64_t* total) {
 
 inline int trace_words(int T) { return 16 * (T > 0 ? T : 0) + 16 + 4 * MAX_ITEMS * 8 + 16; }
 
+// co-resident CTAs of the forward kernel on the current device (computed once per device; a MIG instance or an H100 PCIe
+// has fewer SMs than the 132 of an H100 SXM).  Also opts the kernel into the full 227 KB of shared memory on that device.
+constexpr int MAX_DEVICES = 64;
+int decoder_fwd_capacity(int* out) {
+    static int cap[MAX_DEVICES];
+    int dev = 0;
+    TACO_CUDA(cudaGetDevice(&dev));
+    TACO_CHECK(dev >= 0 && dev < MAX_DEVICES, "taco_decoder: device %d out of range", dev);
+    if (cap[dev] == 0) {
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        int per_sm = 0, sms = 0;
+        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_kernel<false>, NTHR, 227 * 1024));
+        TACO_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        cap[dev] = per_sm * sms > 0 ? per_sm * sms : -1;
+    }
+    *out = cap[dev] > 0 ? cap[dev] : 0;
+    return 0;
+}
+
 }  // namespace
+
+int decoder_bwd_capacity(int* out);     // decoder_bwd.cu
+
+extern "C" int taco_decoder_capacity(int* fwd_ctas, int* bwd_ctas) {
+    int f = 0, b = 0;
+    if (decoder_fwd_capacity(&f) || decoder_bwd_capacity(&b)) return 1;
+    if (fwd_ctas) *fwd_ctas = f;
+    if (bwd_ctas) *bwd_ctas = b;
+    return 0;
+}
 
 extern "C" size_t taco_decoder_packed_bytes(int r) {
     SegDesc sd[NSEG]; int64_t tot;
@@ -975,6 +1008,8 @@ extern "C" int taco_decoder_pack(const taco_decoder_weights* w, int r, float* pa
 
 extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     TACO_CHECK(a, "taco_decoder_fwd: NULL args");
+    TACO_CHECK(a->max_ctas == 0 || a->max_ctas >= NS, "taco_decoder_fwd: max_ctas=%d: the budget must be 0 (the device's capacity) "
+               "or at least %d CTAs", a->max_ctas, NS);
     TACO_CHECK(a->weights != nullptr, "taco_decoder_fwd: weights (biases, attention_v) is NULL");
     const taco_decoder_weights& W = *a->weights;
     TACO_CHECK(a->B >= 1 && a->B <= BPAD, "taco_decoder_fwd: B=%d must be in [1,%d] per launch", a->B, BPAD);
@@ -987,6 +1022,8 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     if (a->mode != TACO_DEC_INFER) TACO_CHECK(a->mel != nullptr, "taco_decoder_fwd: teacher/sched mode needs mel");
     if (a->mode == TACO_DEC_SCHED) TACO_CHECK(a->sample_mask != nullptr, "taco_decoder_fwd: sched mode needs sample_mask");
     TACO_CHECK((a->keep1 == nullptr) == (a->keep2 == nullptr), "taco_decoder_fwd: keep1/keep2 must both be set or both NULL");
+    TACO_CHECK(a->row0 >= 0 && (a->row_stride == 0 ? a->row0 == 0 : a->row0 + a->B <= a->row_stride),
+               "taco_decoder_fwd: rows [%d, %d) outside a row stride of %d", a->row0, a->row0 + a->B, a->row_stride);
     cudaStream_t st = (cudaStream_t)stream;
 
     static DecParams P;                                  // (kept off the stack; a decoder launch is not re-entrant)
@@ -996,6 +1033,7 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     build_ws_layout(P.buf, &P.att_off, &ws_total);
     P.trace_off = ws_total;
     P.a = *a;
+    if (P.a.row_stride == 0) P.a.row_stride = a->B;
     P.OUT = MF * a->r;
     P.NCY = (P.OUT + NS - 1) / NS;
     P.Tq = (a->Tx + 3) / 4;            // quarter width; the last quarter is ragged when Tx % 4 != 0
@@ -1039,30 +1077,28 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     P.smem_total_floats = off + res;
     const size_t smem_bytes = (size_t)P.smem_total_floats * 4;
 
-    static bool configured = false;
-    if (!configured) {
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        configured = true;
-    }
+    // ---- launch geometry: 32 CTAs per row group, as many row groups as the CTA budget allows (at most 4); rows past B are
+    //      padding.  (Sizing the grid to ceil(B/8) row groups instead was measured slower: at B = 1, T = 100 the decoder
+    //      took 1.86 ms on 32 CTAs against 1.82 ms on 128, H100 80GB HBM3 at 400 W.)  Every CTA polls its row group's peers
+    //      (a peer that never runs ends in __trap), so a grid that does not cover the row groups of the launch's
+    //      utterances is refused here ----
+    int capacity = 0;
+    if (decoder_fwd_capacity(&capacity)) return 1;
+    TACO_CHECK(capacity >= NS, "taco_decoder_fwd: only %d CTAs can be co-resident on this device (need %d)", capacity, NS);
+    const int ctas = a->max_ctas > 0 && a->max_ctas < capacity ? a->max_ctas : capacity;
+    const int groups = ctas / NS < NCTA / NS ? ctas / NS : NCTA / NS;
+    TACO_CHECK(groups * RPG >= a->B,
+               "taco_decoder_fwd: B=%d needs %d CTAs (%d row groups of 8 utterances), the budget allows %d: split the batch",
+               a->B, (a->B + RPG - 1) / RPG * NS, (a->B + RPG - 1) / RPG, ctas);
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(NCTA); cfg.blockDim = dim3(NTHR); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = st;
-    // all 128 CTAs must be co-resident (one per SM): the kernel is a dataflow machine without a grid barrier.  A cooperative
+    cfg.gridDim = dim3(groups * NS); cfg.blockDim = dim3(NTHR); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = st;
+    // all CTAs must be co-resident (one per SM): the kernel is a dataflow machine without a grid barrier.  A cooperative
     // launch makes that a guarantee (the launch fails instead of leaving CTAs to spin on peers that never start).
     cudaLaunchAttribute coop;
     coop.id = cudaLaunchAttributeCooperative;
     coop.val.cooperative = 1;
     cfg.attrs = &coop; cfg.numAttrs = 1;
-    static int max_ctas = -1;
-    if (max_ctas < 0) {
-        int per_sm = 0, dev = 0, sms = 0;
-        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_kernel<false>, NTHR, 227 * 1024));
-        TACO_CUDA(cudaGetDevice(&dev));
-        TACO_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        max_ctas = per_sm * sms;
-    }
-    TACO_CHECK(max_ctas >= NCTA, "taco_decoder_fwd: only %d CTAs can be co-resident on this device (need %d)", max_ctas, NCTA);
     TACO_CUDA(cudaMemsetAsync(a->workspace, 0, (size_t)ws_total * 8, st));
     static const bool trace_build = getenv("TACO_TRACE") != nullptr;     // per-stage clock trace (scripts/dec_time.py)
     if (trace_build && a->step_ns) TACO_CUDA(cudaLaunchKernelEx(&cfg, decoder_kernel<true>, P));

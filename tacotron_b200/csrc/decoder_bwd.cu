@@ -145,6 +145,23 @@ __host__ __device__ inline void cta_columns(int N, int G, int cta, bool reverse,
 
 __host__ __device__ inline int side_gemm_ctas(int G, int B) { return (G >= 2 * B) ? G - B : G; }
 
+// the 9 GEMMs of a step (weight-row cache slots): output columns N and contraction length K
+constexpr int GEMM_N[NGEMM] = {256, U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 640};
+constexpr int GEMM_K[NGEMM] = {128, 768, U, 2 * U, U, 2 * U, U, 2 * U, U};
+constexpr size_t SMEM_LIMIT = 200 * 1024;                 // dynamic shared memory the kernel may take
+constexpr size_t SMEM_PARTIALS = ((size_t)NW * CB * 32 + CB * 32) * 4;
+
+// floats of one CTA's weight-row cache on a grid of G CTAs: ceil(N / ctas) rows of K per GEMM (the largest share any CTA
+// gets; cta_columns deals the columns of GEMM 0 over the side_gemm_ctas(G, B) CTAs, every other GEMM over all G)
+inline size_t cache_floats(int G, int B) {
+    size_t f = 0;
+    for (int g = 0; g < NGEMM; ++g) {
+        const int ctas = (g == 0) ? side_gemm_ctas(G, B) : G;
+        f += (size_t)(((GEMM_N[g] + ctas - 1) / ctas) * GEMM_K[g] + 3) & ~(size_t)3;
+    }
+    return f;
+}
+
 // out[row][n] = sum_k in[row][k] * W[n][k] for this CTA's columns, then the stage epilogue per (row, column).
 // pre(row, n) runs BEFORE the product and returns the saved activations / carries the epilogue of (row, n) needs: those L2
 // loads then travel together with the GEMM's input loads instead of after the reduction.
@@ -154,7 +171,7 @@ __device__ __forceinline__ void skinny_gemm(float* part_s, const float* in, int 
                                             int N, int geff, const float* wc, PreF pre, Epi epi) {
     int n0, n1;
     cta_columns(N, geff, (int)blockIdx.x, false, n0, n1);    // geff < grid: only the first geff CTAs take columns
-    for (int nb = n0; nb < n1; nb += CB) {               // one block on the GPU (<= 6 columns per CTA at 128 CTAs)
+    for (int nb = n0; nb < n1; nb += CB) {               // one block at 128 CTAs (<= 6 columns per CTA), up to three at 32
         const int nc = (n1 - nb < CB) ? n1 - nb : CB;
         const int tid = threadIdx.x;
         Pre pr = {0.f, 0.f, 0.f, 0.f, 0.f};
@@ -213,7 +230,7 @@ __global__ void __launch_bounds__(256, 1) decoder_bwd_kernel(const DecBwdP p) {
     const float* wcp[NGEMM];
     {
         const float* Wm[NGEMM] = {p.W2, p.M124, p.Wc[2], p.Wg[2], p.Wc[1], p.Wg[1], p.Wc[0], p.Wg[0], p.M7};
-        const int Nn[NGEMM] = {256, U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 640};
+        const int Nn[NGEMM] = {256, U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 640};     // = GEMM_N, GEMM_K (host)
         const int Kk[NGEMM] = {128, 768, U, 2 * U, U, 2 * U, U, 2 * U, U};
         float* cur = dyn_s + NW * CB * 32 + CB * 32;
         for (int g = 0; g < NGEMM; ++g) {
@@ -458,11 +475,34 @@ __global__ void dy_tail_kernel(float* DY, const float* __restrict__ DX, const ui
 
 }  // namespace
 
+#ifndef TACO_HOST_EMU
+// co-resident CTAs of the backward kernel on the current device (computed once per device); also opts the kernel into
+// SMEM_LIMIT bytes of dynamic shared memory there.  Used by taco_decoder_capacity (decoder.cu).
+int decoder_bwd_capacity(int* out) {
+    constexpr int MAX_DEVICES = 64;
+    static int cap[MAX_DEVICES];
+    int dev = 0;
+    TACO_CUDA(cudaGetDevice(&dev));
+    TACO_CHECK(dev >= 0 && dev < MAX_DEVICES, "taco_decoder_bwd: device %d out of range", dev);
+    if (cap[dev] == 0) {
+        TACO_CUDA(cudaFuncSetAttribute(decoder_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT));
+        int sms = 0, per_sm = 0;
+        TACO_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_bwd_kernel, 256, SMEM_LIMIT));
+        cap[dev] = sms * per_sm > 0 ? sms * per_sm : -1;
+    }
+    *out = cap[dev] > 0 ? cap[dev] : 0;
+    return 0;
+}
+#endif
+
 extern "C" size_t taco_decoder_bwd_workspace_bytes(void) { return (size_t)WS_TOTAL * 4; }
 
 extern "C" int taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream) {
     TACO_CHECK(a, "taco_decoder_bwd: NULL args");
     TACO_CHECK(a->B >= 1 && a->B <= RB, "taco_decoder_bwd: B=%d must be in [1,%d] per launch", a->B, RB);
+    TACO_CHECK(a->max_ctas == 0 || a->max_ctas >= 32, "taco_decoder_bwd: max_ctas=%d: the budget must be 0 (the device's "
+               "capacity) or at least 32 CTAs", a->max_ctas);
     TACO_CHECK(a->T >= 1 && a->Tx >= 1 && a->Tx <= 256, "taco_decoder_bwd: T=%d Tx=%d (Tx <= 256)", a->T, a->Tx);
     TACO_CHECK(a->r >= 1 && 80 * a->r <= MAXK && ((80 * a->r) % 4) == 0, "taco_decoder_bwd: r=%d unsupported", a->r);
     TACO_CHECK(a->W_a && a->W_q && a->W_out && a->W_in && a->W1 && a->W2 && a->v, "taco_decoder_bwd: NULL weight");
@@ -485,6 +525,17 @@ extern "C" int taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream) {
     p.ws = a->workspace;
     p.bar = reinterpret_cast<unsigned int*>(a->workspace + WS_BAR);
     TACO_CHECK(a->T <= WS_MAXT, "taco_decoder_bwd: T=%d exceeds %d steps per launch", a->T, WS_MAXT);
+#ifndef TACO_HOST_EMU
+    // grid: G = min(budget, capacity, 128) CTAs; every CTA takes its columns from gridDim, so any G works.  The weight-row
+    // cache is kept whenever it fits at that G (about 48 KB at 128 CTAs, 62 KB at 114, 98 KB at 64; not at 32)
+    int capacity = 0;
+    if (decoder_bwd_capacity(&capacity)) return 1;
+    TACO_CHECK(capacity >= 32, "taco_decoder_bwd: only %d CTAs can be co-resident on this device (need 32)", capacity);
+    int G = capacity < 128 ? capacity : 128;
+    if (a->max_ctas > 0 && a->max_ctas < G) G = a->max_ctas;
+    p.cache_weights = (SMEM_PARTIALS + cache_floats(G, a->B) * 4 <= SMEM_LIMIT) ? 1 : 0;
+    const size_t smem = SMEM_PARTIALS + (p.cache_weights ? cache_floats(G, a->B) * 4 : 0);
+#endif
     const int OUTh = 80 * a->r, MF = 80, lo = OUTh - MF;
     const int M = a->T * a->B;
     float* M124 = a->workspace + WS_M124;
@@ -532,28 +583,6 @@ extern "C" int taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream) {
     return 0;
 #else
     cudaStream_t st = (cudaStream_t)stream;
-    // dynamic smem: partial sums + the weight rows of one CTA at the grid size used (128 CTAs): ceil(N/128) * K per GEMM
-    const int Nn[NGEMM] = {256, U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 2 * U, 640};
-    const int Kk[NGEMM] = {128, 768, U, 2 * U, U, 2 * U, U, 2 * U, U};
-    size_t cache_floats = 0;
-    for (int g = 0; g < NGEMM; ++g) {
-        const int ctas = (g == 0) ? side_gemm_ctas(128, a->B) : 128;
-        cache_floats += (size_t)(((Nn[g] + ctas - 1) / ctas) * Kk[g] + 3) & ~(size_t)3;
-    }
-    const size_t smem = ((size_t)NW * CB * 32 + CB * 32 + cache_floats) * 4;
-    TACO_CHECK(smem <= 200 * 1024, "taco_decoder_bwd: weight-row cache of %zu bytes does not fit", smem);
-    static int max_ctas = 0;
-    if (max_ctas == 0) {
-        TACO_CUDA(cudaFuncSetAttribute(decoder_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        int dev = 0, sms = 0, per_sm = 0;
-        TACO_CUDA(cudaGetDevice(&dev));
-        TACO_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_bwd_kernel, 256, 200 * 1024));
-        TACO_CHECK(per_sm >= 1, "taco_decoder_bwd: kernel does not fit on an SM");
-        max_ctas = sms * per_sm;
-    }
-    const int G = max_ctas < 128 ? max_ctas : 128;
-    p.cache_weights = (G == 128) ? 1 : 0;                // the cache is sized for 128 CTAs
     TACO_CUDA(cudaMemcpyAsync(M7, a->W_in, (size_t)384 * U * 4, cudaMemcpyDeviceToDevice, st));
     // carries and the stage-4' input start at zero; dattn(T-1) = dctx(T-1) = 0 (the last attention state feeds nothing)
     TACO_CUDA(cudaMemsetAsync(a->workspace, 0, (size_t)WS_ZERO_END * 4, st));

@@ -328,8 +328,17 @@ def decoder_bwd(a):
             getattr(d, k)[i] = a[k][i].data_ptr()
     ws = torch.empty(L.lib().taco_decoder_bwd_workspace_bytes() // 4, dtype=torch.float32, device=a["dy_ext"].device)
     d.workspace = ws.data_ptr()
+    d.max_ctas = int(a.get("max_ctas") or 0)                 # CTA budget, 0 = the device's capacity
     L.check(L.lib().taco_decoder_bwd(C.byref(d), _st()), "taco_decoder_bwd")
     a["_ws"] = ws                                            # keep the scratch alive until the stream has consumed it
+
+
+def decoder_capacity():
+    """(forward, backward): the co-resident CTAs of the two persistent decoder kernels on the current device.  The forward
+    runs 32 CTAs per row group of 8 utterances (at most 4 row groups per launch), the backward min(budget, capacity, 128)."""
+    f, b = C.c_int(0), C.c_int(0)
+    L.check(L.lib().taco_decoder_capacity(C.byref(f), C.byref(b)), "taco_decoder_capacity")
+    return f.value, b.value
 
 
 def attn_bwd_post(dkeys, dv, DSCORE, keys, PQ, v):

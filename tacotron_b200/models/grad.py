@@ -364,7 +364,7 @@ def decoder_bwd(K, P, G, S, cfg, dY_ext):
         "text_length": S["text_length"],
         "DATT": tm(256), "DY": tm(OUT), "DPQ": tm(256), "DSCORE": K.empty((B, T, Tx), like), "DCTX": tm(256),
         "DG": [tm(2 * U) for _ in range(3)], "DC": [tm(U) for _ in range(3)], "DZ": tm(U), "DPN2": tm(128), "DPN1": tm(256),
-        "DX": tm(mf),
+        "DX": tm(mf), "max_ctas": getattr(cfg, "max_ctas", None),
     }
     K.decoder_bwd(a)
     if "_capture" in S:                                   # tests: expose the serial kernel's arguments and outputs

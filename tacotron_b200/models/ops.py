@@ -502,14 +502,69 @@ def _decoder_weights(sc):
     return w
 
 
+# launch geometry of the forward decoder kernel (csrc/decoder.cu): a row group of 8 utterances runs on 32 co-resident CTAs
+# (one per SM), a launch runs as many independent row groups as the CTA budget allows, up to 4 (32 utterances, the size of
+# its workspace), also when it has fewer utterances: a grid sized to the utterances was measured slower (see DESIGN.md)
+DEC_GROUP_ROWS = 8
+DEC_GROUP_CTAS = 32
+DEC_MAX_GROUPS = 4
+
+
+def decoder_budget(capacity, max_ctas=None):
+    """CTAs the decoder kernels may use: the device's co-resident `capacity`, capped by `max_ctas` (None or 0 = no cap).
+    Raises TacoError, before anything is launched, for a cap below one row group or a device that cannot hold one."""
+    if max_ctas is not None and max_ctas != 0 and max_ctas < DEC_GROUP_CTAS:
+        raise L.TacoError(f"max_ctas={max_ctas}: the decoder kernels need at least {DEC_GROUP_CTAS} CTAs (None = the device's capacity)")
+    if capacity < DEC_GROUP_CTAS:
+        raise L.TacoError(f"only {capacity} decoder CTAs can be co-resident on this device; the decoder needs {DEC_GROUP_CTAS}")
+    return capacity if not max_ctas else min(int(max_ctas), capacity)
+
+
+def decoder_plan(B, capacity, max_ctas=None):
+    """The forward decoder launches for B utterances: [(b0, nb, ctas)], utterances b0..b0+nb-1 on `ctas` CTAs.  Each launch
+    runs the row groups the budget allows (min(4, budget // 32) groups of 32 CTAs) and takes up to 8 utterances per group."""
+    groups = min(DEC_MAX_GROUPS, decoder_budget(capacity, max_ctas) // DEC_GROUP_CTAS)
+    rows = DEC_GROUP_ROWS * groups
+    return [(b0, min(rows, B - b0), DEC_GROUP_CTAS * groups) for b0 in range(0, B, rows)]
+
+
+def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stream):
+    """One taco_decoder_fwd per entry of `plan` over the full-batch tensors `t` (dict: packed, keys, values, text_length,
+    y, align, workspace, and mel, sample_mask, keep1, keep2, h_save, step_ns or None).  [B]-major tensors are passed from
+    row b0; the [T][B]-major ones (sample_mask, keep1, keep2, h_save) whole, with row0 = b0 and row_stride = B."""
+    B = t["keys"].shape[0]
+    Tx = t["keys"].shape[1]
+    ptr = lambda x, b0=0: None if x is None else x[b0:].data_ptr()
+    for b0, nb, _ in plan:
+        a = L.DecoderArgs()
+        a.weights = C.pointer(w)
+        a.packed = t["packed"].data_ptr(); a.keys = ptr(t["keys"], b0); a.values = ptr(t["values"], b0)
+        a.text_length = ptr(t["text_length"], b0)
+        a.mode = mode
+        a.mel = ptr(t.get("mel"), b0)
+        a.sample_mask = ptr(t.get("sample_mask")); a.keep1 = ptr(t.get("keep1")); a.keep2 = ptr(t.get("keep2"))
+        a.h_save = ptr(t.get("h_save"))
+        a.row0 = b0; a.row_stride = B
+        a.keep_scale = keep_scale
+        a.B = nb; a.Tx = Tx; a.T = T; a.r = r
+        a.y = ptr(t["y"], b0); a.align = ptr(t["align"], b0); a.workspace = t["workspace"].data_ptr()
+        a.step_ns = ptr(t.get("step_ns"))
+        a.max_ctas = int(max_ctas or 0)
+        L.check(lib.taco_decoder_fwd(C.byref(a), stream), "taco_decoder_fwd")
+
+
 def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sample_mask=None, drop_masks=None,
-                      dropout=0.5, scope=None, step_ns=None):
-    """encoded [B,Tx,256], text_length int32 [B] -> (seq2seq_output [B,T,80r], alignments [B,T,Tx])."""
+                      dropout=0.5, scope=None, step_ns=None, max_ctas=None):
+    """encoded [B,Tx,256], text_length int32 [B] -> (seq2seq_output [B,T,80r], alignments [B,T,Tx]).
+    max_ctas caps the CTAs (SMs) the decoder kernel may occupy (None = all the device holds); the batch is decoded in as
+    many launches of up to 8 x (max_ctas // 32) utterances as it needs (decoder_plan)."""
+    from .. import kernels as K
     sc = scope or current_scope()
     rt = runtime(sc.store)
     B, Tx, D = encoded.shape
     assert D == 256
     lib = L.lib()
+    plan = decoder_plan(B, K.decoder_capacity()[0], max_ctas)     # (raises before any launch for a budget below 32)
     out_w = 80 * r
     y = rt.buf(sc.name("y"), (B, T, out_w))
     align = rt.buf(sc.name("align"), (B, T, Tx))
@@ -532,7 +587,7 @@ def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sa
     ks = 1.0 / (1.0 - dropout)
     hs = None
     if _save is not None:                                        # train: the three GRU state sequences feed the backward
-        assert B <= 32, "training decodes at most 32 utterances per rank (one launch)"
+        assert B <= 32, "training decodes at most 32 utterances per rank (the backward kernel's limit)"
         hs = rt.buf(sc.name("H"), (3, T, B, 256))
         _save[sc.name("H")] = hs; _save[sc.name("values")] = values; _save[sc.name("keys")] = keys
         _save[sc.name("y")] = y; _save[sc.name("align")] = align
@@ -540,29 +595,19 @@ def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sa
             _save[sc.name("keep1")], _save[sc.name("keep2")] = drop_masks
         if mode == L.DEC_SCHED:
             _save[sc.name("sample_mask")] = sample_mask
-    for b0 in range(0, B, 32):                                   # the kernel handles <= 32 utterances per launch
-        nb = min(32, B - b0)
-        a = L.DecoderArgs()
-        a.weights = C.pointer(w)
-        a.packed = packed.data_ptr(); a.keys = keys[b0:].data_ptr(); a.values = values[b0:].data_ptr()
-        a.text_length = text_length[b0:].data_ptr()
-        a.mode = mode
-        if mode != L.DEC_INFER:
-            assert mel is not None and mel.is_contiguous() and mel.shape == (B, T, out_w)
-            a.mel = mel[b0:].data_ptr()
-        if mode == L.DEC_SCHED:
-            assert B <= 32, "scheduled sampling with B > 32 needs a [T, B] mask slice per launch"
-            assert sample_mask is not None and sample_mask.dtype == torch.uint8 and sample_mask.shape == (T, B)
-            a.sample_mask = sample_mask.data_ptr()
-        if drop_masks is not None:
-            assert B <= 32
-            k1, k2 = drop_masks
-            assert k1.dtype == torch.uint8 and k1.shape == (T, B, 256) and k2.shape == (T, B, 128)
-            a.keep1 = k1.data_ptr(); a.keep2 = k2.data_ptr()
-        a.keep_scale = ks
-        a.B = nb; a.Tx = Tx; a.T = T; a.r = r
-        a.y = y[b0:].data_ptr(); a.align = align[b0:].data_ptr(); a.workspace = ws.data_ptr()
-        a.step_ns = step_ns.data_ptr() if step_ns is not None else None
-        a.h_save = hs.data_ptr() if hs is not None else None
-        L.check(lib.taco_decoder_fwd(C.byref(a), L.current_stream()), "taco_decoder_fwd")
+    t = {"packed": packed, "keys": keys, "values": values, "text_length": text_length, "y": y, "align": align,
+         "workspace": ws, "step_ns": step_ns, "h_save": hs}
+    if mode != L.DEC_INFER:
+        assert mel is not None and mel.is_contiguous() and mel.shape == (B, T, out_w)
+        t["mel"] = mel
+    if mode == L.DEC_SCHED:
+        assert sample_mask is not None and sample_mask.dtype == torch.uint8 and sample_mask.shape == (T, B)
+        assert sample_mask.is_contiguous()
+        t["sample_mask"] = sample_mask
+    if drop_masks is not None:
+        k1, k2 = drop_masks
+        assert k1.dtype == torch.uint8 and k1.shape == (T, B, 256) and k2.shape == (T, B, 128)
+        assert k1.is_contiguous() and k2.is_contiguous()
+        t["keep1"], t["keep2"] = k1, k2
+    decoder_fwd_launches(lib, plan, w, t, mode, T, r, ks, max_ctas, L.current_stream())
     return y, align

@@ -50,6 +50,9 @@ class Config(object):
     precision = "fp32x3"
     # replay inference-mode calls from CUDA graphs (captured per input shape)
     cuda_graph = False
+    # CTAs (SMs) the persistent decoder kernels may occupy, at least 32; None = what the device holds.  The forward decodes
+    # 8 x (max_ctas // 32) utterances per launch (up to 32), the backward runs on min(max_ctas, 128) CTAs.
+    max_ctas = None
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -66,6 +69,10 @@ class Tacotron(object):
         if not torch.cuda.is_available():
             raise RuntimeError("tacotron_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         L.lib()                                   # fail loudly if the extension is missing
+        max_ctas = getattr(config, "max_ctas", None)
+        if max_ctas is not None:                  # a budget below one decoder row group fails here, before any launch
+            from .. import kernels as K
+            ops.decoder_budget(K.decoder_capacity()[0], max_ctas)
         self.config = config
         self.train = train
         self.device = torch.device(device)
@@ -131,7 +138,8 @@ class Tacotron(object):
         def run():
             return ops.attention_decoder(encoded, inputs["text_length"], cfg.r, T, mode=mode, mel=mel,
                                          sample_mask=sample_mask, drop_masks=dec_drop_masks,
-                                         dropout=cfg.audio_dropout_prob, scope=sc, step_ns=step_ns)
+                                         dropout=cfg.audio_dropout_prob, scope=sc, step_ns=step_ns,
+                                         max_ctas=getattr(cfg, "max_ctas", None))
         return run
 
     # -- inference (tacotron.py:107-154) --------------------------------------------------------
@@ -205,7 +213,7 @@ class Tacotron(object):
 
     def _inference_graphed(self, inputs, T):
         T = self.config.max_decode_iter if T is None else T
-        key = (tuple(inputs["text"].shape), T, self.store.version)
+        key = (tuple(inputs["text"].shape), T, self.store.version, getattr(self.config, "max_ctas", None))
         g = self._graphs.get(key) if hasattr(self, "_graphs") else None
         if g is None:
             if not hasattr(self, "_graphs"):

@@ -96,12 +96,15 @@ def main(argv=None):
     parser.add_argument("-t", "--train-set", default="nancy")
     parser.add_argument("-s", "--speaker", type=int, default=0, help="speaker id of a multi-speaker model")
     parser.add_argument("--summaries", action="store_true", help="write TensorBoard summaries to log/<save_path>/test")
+    parser.add_argument("--max-ctas", type=int, default=None,
+                        help="CTAs (SMs) the decoder kernels may occupy, at least 32 (default: all the device holds)")
     args = parser.parse_args(argv)
     prompts = [p for p in sys.stdin.readlines() if len(p) > 0]                           # test.py:77-78
     from .models.tacotron import Config, Tacotron
     config = Config()
     config.data_path = "data/%s/" % args.train_set                                       # :83
     config.save_path = args.train_set + "/tacotron"                                      # :84
+    config.max_ctas = args.max_ctas
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "test") if args.summaries else None      # test.py:33
     test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir)

@@ -121,12 +121,15 @@ def main(argv=None):
     parser.add_argument("--steps", type=int, default=1000000)
     parser.add_argument("--summaries", action="store_true", help="write TensorBoard summaries to log/<save_path>/train")
     parser.add_argument("--summary-every", type=int, default=1, help="steps between two per-step summaries")
+    parser.add_argument("--max-ctas", type=int, default=None,
+                        help="CTAs (SMs) the decoder kernels may occupy, at least 32 (default: all the device holds)")
     args = parser.parse_args(argv)
     from .models.tacotron import Config, Tacotron
     config = Config()
     config.data_path = "data/%s/" % args.train_set                                       # train.py:108
     config.restore = args.restore
     config.save_path = "debug" if args.debug else "%s/tacotron" % args.train_set         # :110-113
+    config.max_ctas = args.max_ctas
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "train") if args.summaries else None     # train.py:41
     train(Tacotron, config, num_steps=args.steps, summary_dir=summary_dir, summary_every=args.summary_every)
