@@ -181,6 +181,10 @@ typedef struct taco_decoder_args {
     int32_t        row_stride;   /* row_stride rows per step, this launch's row b is row0 + b (a batch
                                     decoded in several launches); row_stride = 0: B rows, row0 = 0   */
     int32_t        max_ctas;     /* CTA budget (>= 32), 0 = what the device holds (taco_decoder_capacity) */
+    const float*   h0;           /* [3][row_stride][256] initial states of the three GRUs (speaker-conditioned decoder;
+                                    this launch's row b is row0 + b), or NULL = zero state (cell.zero_state)  */
+    const float*   att0;         /* [row_stride][256] initial attention vector, or NULL = zero; needs weights->in_W
+                                    (h0 needs weights->gru_Wg): their step-0 products are formed in the workspace */
 } taco_decoder_args;
 
 int taco_decoder_fwd(const taco_decoder_args* a, void* stream);
@@ -303,6 +307,8 @@ typedef struct taco_decoder_bwd_args {
     float *workspace;                     /* taco_decoder_bwd_workspace_bytes                           */
     int32_t max_ctas;                     /* CTA budget (>= 32), 0 = what the device holds; the kernel runs on
                                              min(budget, capacity, 128) CTAs                                */
+    const float *H0[3];                   /* [B][256] initial state of GRU i (h_i(-1)), or NULL = zero        */
+    float *DH0;                           /* out: [3][B][256] d(loss)/d(h_i(-1)), or NULL = not wanted        */
 } taco_decoder_bwd_args;
 size_t taco_decoder_bwd_workspace_bytes(void);
 int    taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream);

@@ -56,6 +56,7 @@ class DecoderArgs(C.Structure):
         ("y", C.c_void_p), ("align", C.c_void_p), ("workspace", C.c_void_p), ("step_ns", C.c_void_p),
         ("h_save", C.c_void_p),
         ("row0", C.c_int32), ("row_stride", C.c_int32), ("max_ctas", C.c_int32),
+        ("h0", C.c_void_p), ("att0", C.c_void_p),
     ]
 
 
@@ -82,6 +83,7 @@ class DecoderBwdArgs(C.Structure):
         ("DATT", C.c_void_p), ("DY", C.c_void_p), ("DPQ", C.c_void_p), ("DSCORE", C.c_void_p),
         ("DCTX", C.c_void_p), ("DG", C.c_void_p * 3), ("DC", C.c_void_p * 3), ("DZ", C.c_void_p), ("DPN2", C.c_void_p),
         ("DPN1", C.c_void_p), ("DX", C.c_void_p), ("workspace", C.c_void_p), ("max_ctas", C.c_int32),
+        ("H0", C.c_void_p * 3), ("DH0", C.c_void_p),
     ]
 
 

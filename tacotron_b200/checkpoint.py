@@ -64,6 +64,7 @@ def latest_checkpoint(save_path):
 def restore(model, filename):
     """saver.restore(sess, ckpt): parameters, Adam slots, global_step; returns (stft_mean, stft_std) or (None, None)"""
     z = np.load(filename)
+    _check_variables(model, z.files, filename)
     model.load_params({n: torch.from_numpy(z[n]) for n in model.store.shapes})
     model.global_step = int(z["global_step"])
     if "adam/m" in z.files:
@@ -76,6 +77,29 @@ def restore(model, filename):
     return None, None
 
 
+# entries of a checkpoint written by `save` that are not model variables
+_NON_PARAMS = ("global_step", "adam/m", "adam/v", "adam/step", "stft_mean", "stft_std")
+
+
+def _check_variables(model, names, filename):
+    """a checkpoint of a model with the other Config.speaker_decoder setting is refused, naming the variables, instead of
+    being loaded partly (or, for the missing ones, from whatever the model was initialised with)"""
+    if getattr(model, "store", None) is None:            # (a loader without a parameter list: nothing to compare)
+        return
+    have = set(names) - set(_NON_PARAMS)
+    want = set(model.store.shapes)
+    missing, extra = sorted(want - have), sorted(n for n in have - want if n.startswith("dec/spk/"))
+    if extra or any(n.startswith("dec/spk/") for n in missing):
+        raise ValueError(f"{filename} does not match the model (speaker_decoder = "
+                         f"{bool(getattr(getattr(model, 'config', None), 'speaker_decoder', False))}): missing variables {missing}, "
+                         f"extra variables {extra}")
+
+
+def speaker_decoder(filename):
+    """whether a checkpoint written by `save` holds a speaker-conditioned decoder (Config.speaker_decoder)"""
+    return "dec/spk/attn/W" in np.load(filename).files
+
+
 def num_speakers(filename):
     """speaker count of a checkpoint written by `save` (rows of its speaker table; 1 for a single-speaker model)"""
     z = np.load(filename)
@@ -85,16 +109,20 @@ def num_speakers(filename):
 def import_tf_variables(model, tf_vars):
     """{TF-1.2 variable name: ndarray} -> parameter store.  Non-model variables (global_step, Adam slots, stft_mean/std,
     beta1_power ...) are returned in a dict instead of being loaded.  A bundle with a speaker table
-    (``speaker/speaker_embed``) is read with the multi-speaker name map."""
+    (``speaker/speaker_embed``) is read with the multi-speaker name map, one with the decoder's speaker denses
+    (``decoder/dense``) with the speaker-conditioned decoder's."""
     params, extra = {}, {}
     strip = lambda n: n[:-2] if n.endswith(":0") else n
     multi = any(strip(n) == "speaker/speaker_embed" for n in tf_vars)
+    spk_dec = multi and any(strip(n) == "decoder/dense/kernel" for n in tf_vars)
     for name, arr in tf_vars.items():
         name = strip(name)
         try:
-            params[tf_name_to_param(name, multi_speaker=multi)] = torch.from_numpy(np.asarray(arr, dtype=np.float32))
+            params[tf_name_to_param(name, multi_speaker=multi, speaker_decoder=spk_dec)] = \
+                torch.from_numpy(np.asarray(arr, dtype=np.float32))
         except KeyError:
             extra[name] = arr
+    _check_variables(model, params, "the TensorFlow checkpoint")
     model.load_params(params)
     return extra
 

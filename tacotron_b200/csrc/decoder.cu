@@ -123,6 +123,8 @@ struct DecParams {
     taco_decoder_args a;
     const float *in_b, *gru_bg[3], *gru_bc[3], *out_b, *pre_b1, *pre_b2, *att_v;
     const float *b_qF, *b_p1F, *b_inS;     // fused biases (packed tail)
+    const float *init_z, *init_g;          // step-0 terms of a non-zero initial state (workspace tail), or NULL:
+                                           //   att0 . W_in[128:] [32][256],  h0_i . Wg_i[256:] [3][32][512]
     int OUT, NCY, Tq;
     int smem_kv_off, smem_res_off, smem_total_floats;
 };
@@ -337,7 +339,12 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     const int myrow = row0 + g;                        // the utterance row this lane's B fragments belong to
     const int lane_w = g * 8 + 2 * tg;                  // this lane's word offset inside a k-tile block
 
-    for (int i = tid; i < 384; i += NTHR) loc_s[i] = 0.f;          // zero initial GRU states (cell.zero_state)
+    for (int i = tid; i < 384; i += NTHR) {                        // initial GRU states: h0 rows, or zero (cell.zero_state)
+        float hv = 0.f;
+        if (i < 192 && A.h0 && row0 + (i & 7) < B)                 // h_loc[gi][col][row]: unit 8cs + col of row (i & 7)
+            hv = __ldg(A.h0 + ((int64_t)(i >> 6) * RS + R0 + row0 + (i & 7)) * U + 8 * cs + ((i >> 3) & 7));
+        loc_s[i] = hv;
+    }
     // biases of this CTA's columns -> smem
     if (tid < NBR * 16) {
         const int br = tid >> 4, m = tid & 15;
@@ -689,6 +696,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
                 if (tid < 64) {
                     float zv = sum16(part, e_pidx) + bias_s[BR_IN * 16 + e_wc];
                     if (t > 0) zv += bias_s[BR_INX * 16 + e_wc];
+                    else if (P.init_z && e_row < B) zv += P.init_z[e_row * U + 8 * cs + e_wc];      // att0 . W_in[128:]
                     z_loc[e_loc] = zv;
                     ll_store(ws + otab[O_Z] + e_word, zv, tag);
                 }
@@ -696,7 +704,10 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             case ST_G0: case ST_G1: case ST_G2:
                 if (tid < 128) {
                     const int gi = stage - ST_G0;
-                    const float gt = sigmoidf_acc(sum16(part, e_pidx) + bias_s[(BR_G0 + gi) * 16 + e_wc + 8 * e_hi]);
+                    float gp = sum16(part, e_pidx) + bias_s[(BR_G0 + gi) * 16 + e_wc + 8 * e_hi];
+                    if (t == 0 && P.init_g && e_row < B)                                          // h0_i . Wg_i[256:]
+                        gp += P.init_g[((int64_t)gi * BPAD + e_row) * 2 * U + U * e_hi + 8 * cs + e_wc];
+                    const float gt = sigmoidf_acc(gp);
                     if (!e_hi) ll_store(ws + otab[O_RH0 + gi] + e_word, gt * h_loc[gi * 64 + e_loc], tag);   // r * h
                     else u_loc[e_loc] = gt;                                                                // u stays local
                 }
@@ -912,6 +923,8 @@ void build_ws_layout(int64_t* buf, int64_t* att, int64_t* total) {
 }
 
 inline int trace_words(int T) { return 16 * (T > 0 ? T : 0) + 16 + 4 * MAX_ITEMS * 8 + 16; }
+// after the trace: the step-0 terms of an initial state, [32][256] (attention vector) + [3][32][512] (GRU states) floats
+constexpr int64_t INIT_Z_FLOATS = (int64_t)BPAD * U, INIT_FLOATS = INIT_Z_FLOATS + 3 * (int64_t)BPAD * 2 * U;
 
 // co-resident CTAs of the forward kernel on the current device (computed once per device; a MIG instance or an H100 PCIe
 // has fewer SMs than the 132 of an H100 SXM).  Also opts the kernel into the full 227 KB of shared memory on that device.
@@ -955,7 +968,7 @@ extern "C" size_t taco_decoder_workspace_bytes(int B, int Tx, int T, int r) {
     (void)B; (void)Tx; (void)r;
     int64_t buf[NBUF], att, total;
     build_ws_layout(buf, &att, &total);
-    return (size_t)(total + trace_words(T)) * 8;
+    return (size_t)(total + trace_words(T)) * 8 + (size_t)INIT_FLOATS * 4;
 }
 
 extern "C" int taco_decoder_pack(const taco_decoder_weights* w, int r, float* packed, void* stream) {
@@ -1100,6 +1113,33 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     coop.val.cooperative = 1;
     cfg.attrs = &coop; cfg.numAttrs = 1;
     TACO_CUDA(cudaMemsetAsync(a->workspace, 0, (size_t)ws_total * 8, st));
+    // initial state (speaker-conditioned decoder): the kernel skips the h(t-1) and attention products at t = 0, so their
+    // step-0 values att0 . W_in[128:] and h0_i . Wg_i[256:] are formed here, per row of this launch, and added by the IN
+    // and G epilogues of step 0 (the C stage sees h0 through r * h and the state update)
+    if (a->att0 || a->h0) {
+        float* init = reinterpret_cast<float*>(reinterpret_cast<uint64_t*>(a->workspace) + ws_total + trace_words(a->T));
+        const int RS = P.a.row_stride;
+        auto term = [&](const float* X, const float* Wm, int N, float* dst) {     // dst[b][n] = X[b] . Wm[:, n], b < B
+            taco_gemm_desc g;                                                   // (the library's own GEMM)
+            memset(&g, 0, sizeof(g));
+            g.A = X; g.lda = U; g.B = Wm; g.ldb = N; g.C = dst; g.ldc = N; g.M = a->B; g.N = N; g.K = U;
+            g.taps = 1; g.batch = 1;
+            return taco_gemm(&g, stream);
+        };
+        if (a->att0) {
+            TACO_CHECK(W.in_W != nullptr, "taco_decoder_fwd: att0 needs weights->in_W");
+            if (term(a->att0 + (int64_t)a->row0 * U, W.in_W + (int64_t)128 * U, U, init)) return 1;
+            P.init_z = init;
+        }
+        if (a->h0) {
+            for (int i = 0; i < 3; ++i) {
+                TACO_CHECK(W.gru_Wg[i] != nullptr, "taco_decoder_fwd: h0 needs weights->gru_Wg");
+                if (term(a->h0 + ((int64_t)i * RS + a->row0) * U, W.gru_Wg[i] + (int64_t)U * 2 * U, 2 * U,
+                         init + INIT_Z_FLOATS + (int64_t)i * BPAD * 2 * U)) return 1;
+            }
+            P.init_g = init + INIT_Z_FLOATS;
+        }
+    }
     static const bool trace_build = getenv("TACO_TRACE") != nullptr;     // per-stage clock trace (scripts/dec_time.py)
     if (trace_build && a->step_ns) TACO_CUDA(cudaLaunchKernelEx(&cfg, decoder_kernel<true>, P));
     else                           TACO_CUDA(cudaLaunchKernelEx(&cfg, decoder_kernel<false>, P));

@@ -58,6 +58,7 @@ struct DecBwdP {
     const uint8_t* sel;
     float *DATT, *DY, *DPQ, *DSCORE, *DCTX, *DG[3], *DC[3], *DZ, *DPN2, *DPN1, *DX;
     const float *M124, *M7, *E;   // fused weights [U][768], [640][U]; E = dy_ext . W_out^T  [T][B][U]   (workspace, see host)
+    const float* H0[3];           // [B][U] initial states h_i(-1), or NULL (zero state)
     float* ws;
     unsigned int* bar;       // grid-barrier counter (zeroed by the host before the launch)
     int cache_weights;       // 1: this CTA's weight rows fit in shared memory (the normal case); 0: read them from L2
@@ -253,7 +254,7 @@ __global__ void __launch_bounds__(256, 1) decoder_bwd_kernel(const DecBwdP p) {
     auto head_pre = [&](int i, int t, int row, int n, Pre& q) {
         const int64_t o = (int64_t)t * B + row;
         q.x0 = __ldcg(dhc + (i * RB + row) * U + n);
-        q.x1 = (t > 0) ? __ldg(p.Hs[i] + (o - B) * U + n) : 0.f;
+        q.x1 = (t > 0) ? __ldg(p.Hs[i] + (o - B) * U + n) : (p.H0[i] ? __ldg(p.H0[i] + row * U + n) : 0.f);
         q.x2 = __ldg(p.RU[i] + o * 2 * U + U + n);
         q.x3 = __ldg(p.C[i] + o * U + n);
     };
@@ -390,7 +391,8 @@ __global__ void __launch_bounds__(256, 1) decoder_bwd_kernel(const DecBwdP p) {
                         Pre q = pre0;
                         if (row < B && n >= U) {
                             const int64_t o = (int64_t)t * B + row;
-                            q.x0 = (t > 0) ? __ldg(p.Hs[i] + (o - B) * U + (n - U)) : 0.f;
+                            q.x0 = (t > 0) ? __ldg(p.Hs[i] + (o - B) * U + (n - U))
+                                           : (p.H0[i] ? __ldg(p.H0[i] + row * U + (n - U)) : 0.f);
                             q.x1 = __ldg(p.RU[i] + o * 2 * U + (n - U));
                         }
                         return q;
@@ -520,6 +522,7 @@ extern "C" int taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream) {
     }
     p.dy_ext = a->dy_ext; p.align = a->align; p.values = a->values; p.keys = a->keys; p.PQ = a->PQ; p.PN1 = a->PN1; p.PN2 = a->PN2;
     p.sel = a->sel;
+    for (int i = 0; i < 3; ++i) p.H0[i] = a->H0[i];
     p.DATT = a->DATT; p.DY = a->DY; p.DPQ = a->DPQ; p.DSCORE = a->DSCORE; p.DCTX = a->DCTX; p.DZ = a->DZ; p.DPN2 = a->DPN2;
     p.DPN1 = a->DPN1; p.DX = a->DX;
     p.ws = a->workspace;
@@ -574,6 +577,8 @@ extern "C" int taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream) {
     memcpy(a->DY, a->dy_ext, (size_t)M * OUTh * 4);
     emu::launch(dim3(1), dim3(256), [&] { decoder_bwd_kernel(p); });
     ++g_taco_launches;
+    if (a->DH0)                                          // after step 0 the GRU carries are d(loss)/d(h_i(-1))
+        for (int i = 0; i < 3; ++i) memcpy(a->DH0 + (int64_t)i * a->B * U, a->workspace + WS_DHC + (int64_t)i * RB * U, (size_t)a->B * U * 4);
     if (tail()) return 1;
     {
         float* DY = a->DY; const float* DX = a->DX; const uint8_t* sel = a->sel; const int T = a->T, B = a->B;
@@ -592,6 +597,9 @@ extern "C" int taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream) {
     void* args[] = {(void*)&p};
     TACO_CUDA(cudaLaunchCooperativeKernel((void*)decoder_bwd_kernel, dim3(G), dim3(256), args, smem, st));
     ++g_taco_launches;
+    if (a->DH0)                                          // after step 0 the GRU carries are d(loss)/d(h_i(-1))
+        TACO_CUDA(cudaMemcpy2DAsync(a->DH0, (size_t)a->B * U * 4, a->workspace + WS_DHC, (size_t)RB * U * 4, (size_t)a->B * U * 4, 3,
+                                    cudaMemcpyDeviceToDevice, st));
     if (tail()) return 1;
     if (a->T > 1) {
         const int64_t total = (int64_t)(a->T - 1) * a->B * MF;

@@ -326,6 +326,13 @@ def decoder_bwd(a):
         for i in range(3):
             assert a[k][i].is_contiguous(), k
             getattr(d, k)[i] = a[k][i].data_ptr()
+    if a.get("H0") is not None:                              # initial GRU states h_i(-1) [B][256] (speaker-conditioned decoder)
+        for i in range(3):
+            assert a["H0"][i].is_contiguous() and a["H0"][i].is_cuda and tuple(a["H0"][i].shape) == (B, 256)
+            d.H0[i] = a["H0"][i].data_ptr()
+    if a.get("DH0") is not None:                             # out: d(loss)/d(h_i(-1)) [3][B][256]
+        assert a["DH0"].is_contiguous() and a["DH0"].is_cuda and tuple(a["DH0"].shape) == (3, B, 256)
+        d.DH0 = a["DH0"].data_ptr()
     ws = torch.empty(L.lib().taco_decoder_bwd_workspace_bytes() // 4, dtype=torch.float32, device=a["dy_ext"].device)
     d.workspace = ws.data_ptr()
     d.max_ctas = int(a.get("max_ctas") or 0)                 # CTA budget, 0 = the device's capacity

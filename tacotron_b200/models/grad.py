@@ -312,9 +312,13 @@ def decoder_recompute(K, P, S, cfg):
     R["ATT"] = ATT
     # InputProjectionWrapper: z(t) = [pn2(t), attn(t-1)] . W_in + b_in
     W_in = P["dec/in_proj/W"]
+    h0, att0 = S.get("dec/h0"), S.get("dec/att0")                              # speaker-conditioned decoder: h_i(-1), a(-1)
+    R["h0"], R["att0"] = h0, att0
     Z = K.empty((M, U), y)
     K.gemm(Z, PN2, W_in[:128])
     K.gemm(Z, ATT, W_in[128:], beta=1.0, shift=-B)
+    if att0 is not None:                                                       # step 0 rows: a(-1) instead of zero
+        K.gemm(Z[:B], att0, W_in[128:], beta=1.0)
     K.bias_act_(Z, P["dec/in_proj/b"], ACT_NONE)
     R["Z"] = Z
     # the three GRU layers: gates from the saved state sequences
@@ -326,9 +330,13 @@ def decoder_recompute(K, P, S, cfg):
         RU = K.empty((M, 2 * U), y)
         K.gemm(RU, inp, Wg[:U])
         K.gemm(RU, Hi, Wg[U:], beta=1.0, shift=-B)
+        if h0 is not None:                                                     # step 0 rows: h_i(-1) instead of zero
+            K.gemm(RU[:B], h0[i], Wg[U:], beta=1.0)
         K.bias_act_(RU, P[f"dec/gru{i+1}/bg"], ACT_SIGMOID)
         RHm = K.empty((M, U), y)
         K.mul_shift(RHm, RU[:, :U], Hi, -B, 0)
+        if h0 is not None:
+            K.mul_shift(RHm[:B], RU[:B, :U], h0[i], 0, 0)
         Cc = K.empty((M, U), y)
         K.gemm(Cc, inp, Wc[:U])
         K.gemm(Cc, RHm, Wc[U:], beta=1.0)
@@ -366,6 +374,10 @@ def decoder_bwd(K, P, G, S, cfg, dY_ext):
         "DG": [tm(2 * U) for _ in range(3)], "DC": [tm(U) for _ in range(3)], "DZ": tm(U), "DPN2": tm(128), "DPN1": tm(256),
         "DX": tm(mf), "max_ctas": getattr(cfg, "max_ctas", None),
     }
+    h0, att0 = R["h0"], R["att0"]
+    if h0 is not None:
+        a["H0"] = [h0[i] for i in range(3)]
+        a["DH0"] = K.empty((3, B, U), like)
     K.decoder_bwd(a)
     if "_capture" in S:                                   # tests: expose the serial kernel's arguments and outputs
         S["_capture"]["decoder_bwd"] = a
@@ -390,6 +402,11 @@ def decoder_bwd(K, P, G, S, cfg, dY_ext):
     K.gemm(G["dec/in_proj/W"][:128], R["PN2"], DZ, ta=True, beta=1.0)
     K.gemm(G["dec/in_proj/W"][128:], R["ATT"], DZ, ta=True, beta=1.0, shift=-B)
     K.colsum(G["dec/in_proj/b"], DZ)
+    if h0 is not None:                                                         # step-0 products of the initial state
+        for i in range(3):
+            K.gemm(G[f"dec/gru{i+1}/Wg"][U:], h0[i], _v2(a["DG"][i])[:B], ta=True, beta=1.0)
+        K.gemm(G["dec/in_proj/W"][128:], att0, DZ[:B], ta=True, beta=1.0)
+        decoder_speaker_bwd(K, P, G, S, DZ[:B], a["DH0"])
     DPN2, DPN1 = _v2(a["DPN2"]), _v2(a["DPN1"])
     K.gemm(G["dec/prenet/W2"], R["PN1"], DPN2, ta=True, beta=1.0)
     K.colsum(G["dec/prenet/b2"], DPN2)
@@ -407,6 +424,25 @@ def decoder_bwd(K, P, G, S, cfg, dY_ext):
     dEnc = K.empty((B, Tx, 256), like)
     K.mask_rows(dEnc, dvalues, S["text_length"])
     return dEnc
+
+
+def decoder_speaker_bwd(K, P, G, S, DZ0, DH0):
+    """Reverse of ops.decoder_speaker_state: S = e.[Wa | Wh1 | Wh2 | Wh3] + b, relu on the three state blocks, e = speaker
+    table rows of S['speaker'].  DZ0 [B,256] = d(loss)/d(z(0)), DH0 [3,B,256] = d(loss)/d(h_i(-1)) (taco_decoder_bwd)."""
+    Sv, e = S["dec/spk_s"], S["dec/spk_e"]
+    B = Sv.shape[0]
+    W_in = P["dec/in_proj/W"]
+    dSv = K.empty(Sv.shape, Sv)
+    K.gemm(dSv[:, :256], DZ0, W_in[128:], tb=True)                             # d a(-1) = dz(0) . W_in[128:]^T
+    dSv[:, 256:].view(B, 3, 256).copy_(DH0.transpose(0, 1))                     # (data movement)
+    K.epi_bwd(dSv[:, 256:], dSv[:, 256:], Sv[:, 256:], True)                   # relu of the state blocks
+    de = K.empty(e.shape, e)
+    for i, nm in enumerate(("attn", "h1", "h2", "h3")):
+        blk = dSv[:, 256 * i:256 * (i + 1)]
+        K.gemm(G[f"dec/spk/{nm}/W"], e, blk, ta=True, beta=1.0)
+        K.colsum(G[f"dec/spk/{nm}/b"], blk)
+        K.gemm(de, blk, P[f"dec/spk/{nm}/W"], tb=True, beta=0.0 if i == 0 else 1.0)
+    K.scatter_add_rows(G["speaker/embed"], S["speaker"], de)
 
 
 # ------------------------------------------------------------------------------------------------------------

@@ -489,6 +489,42 @@ class InferenceHelper:
 # ----------------------------------------------------------------------------------------------
 # attention decoder (models/tacotron.py:46-105,136-138): one persistent kernel for all T steps
 # ----------------------------------------------------------------------------------------------
+def decoder_speaker_state(sc, e):
+    """Speaker conditioning of the decoder (Config.speaker_decoder) from e [B,16]: the initial attention vector
+    a(-1) = e.Wa + ba (the reference's commented-out line, models/tacotron.py:96-97) and the initial GRU states
+    h_i(-1) = relu(e.Wh_i + bh_i), as ONE contraction S = e.[Wa | Wh1 | Wh2 | Wh3] + b with the relu on the three state
+    blocks.  Returns (S [B,1024], h0 [3,B,256], att0 [B,256]); h0 / att0 contiguous, the decoder kernel's layouts."""
+    rt = runtime(sc.store)
+    B, E = e.shape
+    names = ("attn", "h1", "h2", "h3")
+
+    def build_w(old):
+        w = torch.cat([sc.p(f"spk/{n}/W") for n in names], dim=1)
+        if old is not None:
+            old.copy_(w); return old
+        return w.contiguous()
+
+    def build_b(old):
+        b = torch.cat([sc.p(f"spk/{n}/b") for n in names])
+        if old is not None:
+            old.copy_(b); return old
+        return b.contiguous()
+    Ws = rt.get(("spk_w", sc.prefix), build_w)
+    bs = rt.get(("spk_b", sc.prefix), build_b)
+    NS = 256 * len(names)
+    Sv = linear(rt, e.view(1, B, E), Ws, packed_weight(rt, sc.name("spk_w"), Ws, 1, E, NS), NS, bias=bs,
+                tag=sc.name("spk_s")).view(B, NS)
+    L.check(L.lib().taco_bias_act(C.c_void_p(Sv.data_ptr() + 256 * 4), NS, B, NS - 256, None, L.ACT_RELU, L.current_stream()),
+            "taco_bias_act")
+    h0 = rt.buf(sc.name("spk_h0"), (3, B, 256))
+    h0.copy_(Sv[:, 256:].view(B, 3, 256).transpose(0, 1))           # the kernel reads [3][B][256] (data movement only)
+    att0 = rt.buf(sc.name("spk_att0"), (B, 256))
+    att0.copy_(Sv[:, :256])
+    if _save is not None:
+        _save[sc.name("spk_e")] = e; _save[sc.name("spk_s")] = Sv; _save[sc.name("h0")] = h0; _save[sc.name("att0")] = att0
+    return Sv, h0, att0
+
+
 def _decoder_weights(sc):
     w = L.DecoderWeights()
     w.pre_W1 = sc.p("prenet/W1").data_ptr(); w.pre_b1 = sc.p("prenet/b1").data_ptr()
@@ -530,8 +566,9 @@ def decoder_plan(B, capacity, max_ctas=None):
 
 def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stream):
     """One taco_decoder_fwd per entry of `plan` over the full-batch tensors `t` (dict: packed, keys, values, text_length,
-    y, align, workspace, and mel, sample_mask, keep1, keep2, h_save, step_ns or None).  [B]-major tensors are passed from
-    row b0; the [T][B]-major ones (sample_mask, keep1, keep2, h_save) whole, with row0 = b0 and row_stride = B."""
+    y, align, workspace, and mel, sample_mask, keep1, keep2, h_save, step_ns, h0, att0 or None).  [B]-major tensors are
+    passed from row b0; the [T][B]-major ones (sample_mask, keep1, keep2, h_save) and the initial states h0 [3][B][256],
+    att0 [B][256] whole, with row0 = b0 and row_stride = B."""
     B = t["keys"].shape[0]
     Tx = t["keys"].shape[1]
     ptr = lambda x, b0=0: None if x is None else x[b0:].data_ptr()
@@ -549,13 +586,15 @@ def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stre
         a.B = nb; a.Tx = Tx; a.T = T; a.r = r
         a.y = ptr(t["y"], b0); a.align = ptr(t["align"], b0); a.workspace = t["workspace"].data_ptr()
         a.step_ns = ptr(t.get("step_ns"))
+        a.h0 = ptr(t.get("h0")); a.att0 = ptr(t.get("att0"))
         a.max_ctas = int(max_ctas or 0)
         L.check(lib.taco_decoder_fwd(C.byref(a), stream), "taco_decoder_fwd")
 
 
 def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sample_mask=None, drop_masks=None,
-                      dropout=0.5, scope=None, step_ns=None, max_ctas=None):
+                      dropout=0.5, scope=None, step_ns=None, max_ctas=None, h0=None, att0=None):
     """encoded [B,Tx,256], text_length int32 [B] -> (seq2seq_output [B,T,80r], alignments [B,T,Tx]).
+    h0 [3,B,256] / att0 [B,256]: initial GRU states / attention vector (speaker-conditioned decoder), None = zero.
     max_ctas caps the CTAs (SMs) the decoder kernel may occupy (None = all the device holds); the batch is decoded in as
     many launches of up to 8 x (max_ctas // 32) utterances as it needs (decoder_plan)."""
     from .. import kernels as K
@@ -596,7 +635,11 @@ def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sa
         if mode == L.DEC_SCHED:
             _save[sc.name("sample_mask")] = sample_mask
     t = {"packed": packed, "keys": keys, "values": values, "text_length": text_length, "y": y, "align": align,
-         "workspace": ws, "step_ns": step_ns, "h_save": hs}
+         "workspace": ws, "step_ns": step_ns, "h_save": hs, "h0": h0, "att0": att0}
+    if h0 is not None:
+        assert h0.shape == (3, B, 256) and h0.is_contiguous()
+    if att0 is not None:
+        assert att0.shape == (B, 256) and att0.is_contiguous()
     if mode != L.DEC_INFER:
         assert mel is not None and mel.is_contiguous() and mel.shape == (B, T, out_w)
         t["mel"] = mel

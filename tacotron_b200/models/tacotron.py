@@ -53,6 +53,8 @@ class Config(object):
     # CTAs (SMs) the persistent decoder kernels may occupy, at least 32; None = what the device holds.  The forward decodes
     # 8 x (max_ctas // 32) utterances per launch (up to 32), the backward runs on min(max_ctas, 128) CTAs.
     max_ctas = None
+    # multi-speaker models: condition the decoder on the speaker too (initial attention vector and GRU states, DESIGN.md §7)
+    speaker_decoder = False
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -134,12 +136,17 @@ class Tacotron(object):
             sample_mask = None
         sc = ops.Scope(self.store, "dec")
         step_ns = self.step_ns
+        if speaker_embed is not None and not getattr(cfg, "speaker_decoder", False):
+            raise ValueError("speaker_embed given to create_decoder of a model without speaker_decoder")
 
         def run():
+            h0 = att0 = None
+            if speaker_embed is not None:                     # initial attention vector and GRU states (tacotron.py:96-97)
+                _, h0, att0 = ops.decoder_speaker_state(sc, speaker_embed)
             return ops.attention_decoder(encoded, inputs["text_length"], cfg.r, T, mode=mode, mel=mel,
                                          sample_mask=sample_mask, drop_masks=dec_drop_masks,
                                          dropout=cfg.audio_dropout_prob, scope=sc, step_ns=step_ns,
-                                         max_ctas=getattr(cfg, "max_ctas", None))
+                                         max_ctas=getattr(cfg, "max_ctas", None), h0=h0, att0=att0)
         return run
 
     # -- inference (tacotron.py:107-154) --------------------------------------------------------
@@ -160,6 +167,13 @@ class Tacotron(object):
         L.check(L.lib().taco_gather_rows(L.ptr(table), L.ptr(spk), B, table.shape[1], table.shape[0], None, 1.0, L.ptr(e),
                                          L.current_stream()), "taco_gather_rows")
         return e
+
+    def _decoder_speaker_embed(self, B):
+        """e [B,16] for a speaker-conditioned decoder: the rows the encoder gathered in this call (_speaker_embed's buffer,
+        also the CUDA-graph path's static one), or None"""
+        if not getattr(self.config, "speaker_decoder", False):
+            return None
+        return self.runtime.buf("speaker/e", (B, self.store["speaker/embed"].shape[1]))
 
     def _encoder(self, inputs, train, enc_drop_masks, trace):
         cfg, store = self.config, self.store
@@ -204,7 +218,8 @@ class Tacotron(object):
         encoded = self._encoder(inputs, train, enc_drop_masks, trace)
         self._mark("encoder")
         # attention decoder (:135-138)
-        dec = self.create_decoder(encoded, inputs, None, train, T=T, dec_drop_masks=dec_drop_masks, sample_mask=sample_mask)
+        dec = self.create_decoder(encoded, inputs, self._decoder_speaker_embed(B), train, T=T, dec_drop_masks=dec_drop_masks,
+                                  sample_mask=sample_mask)
         seq2seq_output, self.alignments = dec()
         self._mark("decoder")
         output = self._postnet(seq2seq_output, trace)
@@ -236,7 +251,8 @@ class Tacotron(object):
                     outs["encoded"] = self._encoder(static, False, None, None)
                 gd = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(gd, pool=pool):
-                    dec = self.create_decoder(outs["encoded"], static, None, False, T=T)
+                    dec = self.create_decoder(outs["encoded"], static, self._decoder_speaker_embed(static["text"].shape[0]),
+                                              False, T=T)
                     outs["y"], outs["align"] = dec()
                 gp = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(gp, pool=pool):

@@ -74,6 +74,10 @@ def model_shapes(cfg):
     P += [("post/dense/W", (256, cfg.fft_size), "dense"), ("post/dense/b", (cfg.fft_size,), "zeros")]
     if getattr(cfg, "num_speakers", 1) > 1:
         P += speaker_shapes(cfg.num_speakers, getattr(cfg, "speaker_embed_dim", 16))
+    if getattr(cfg, "speaker_decoder", False):
+        if getattr(cfg, "num_speakers", 1) <= 1:
+            raise ValueError("speaker_decoder needs a multi-speaker model (num_speakers > 1): there is no speaker embedding")
+        P += decoder_speaker_shapes(getattr(cfg, "speaker_embed_dim", 16), U, A)
     return P
 
 
@@ -87,6 +91,16 @@ def speaker_shapes(num_speakers, E=16, n_hw=4, units=128):
         P += [(f"enc/cbhg/highway{l}/Ws", (E, units), "dense"), (f"enc/cbhg/highway{l}/bs", (units,), "zeros"),
               (f"enc/cbhg/highway{l}/Wd", (2 * units, units), "dense"), (f"enc/cbhg/highway{l}/bd", (units,), "zeros")]
     P += [("enc/cbhg/gru_init/Ws", (E, units), "dense"), ("enc/cbhg/gru_init/bs", (units,), "zeros")]
+    return P
+
+
+def decoder_speaker_shapes(E=16, units=256, attention_units=256):
+    """Speaker conditioning of the decoder (Config.speaker_decoder), stored after the other speaker variables: the dense
+    giving the initial attention vector a(-1) = e.W + b (the reference's commented-out line, models/tacotron.py:96-97) and
+    one dense per decoder GRU giving its initial state h_i(-1) = relu(e.W + b) (the form of ops.py:111-113)."""
+    P = [("dec/spk/attn/W", (E, attention_units), "dense"), ("dec/spk/attn/b", (attention_units,), "zeros")]
+    for i in (1, 2, 3):
+        P += [(f"dec/spk/h{i}/W", (E, units), "dense"), (f"dec/spk/h{i}/b", (units,), "zeros")]
     return P
 
 

@@ -36,6 +36,7 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None):
     tf_ck = None
     if ck is not None:
         config.num_speakers = checkpoint.num_speakers(ck)
+        config.speaker_decoder = checkpoint.speaker_decoder(ck)
     else:
         # no checkpoint of ours: a checkpoint written by the reference itself (TensorFlow V2 format, e.g. the released
         # Nancy weights of download_weights.sh) in the same directory is read directly
@@ -45,6 +46,7 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None):
             raise FileNotFoundError(f"no checkpoint under weights/{config.save_path}")
         spk = tf_checkpoint.read_bundle(tf_ck, names={"speaker/speaker_embed"}).get("speaker/speaker_embed")
         config.num_speakers = 1 if spk is None else int(np.asarray(spk).shape[0])
+        config.speaker_decoder = bool(tf_checkpoint.read_bundle(tf_ck, names={"decoder/dense/kernel"}))
     if not 0 <= speaker < config.num_speakers:
         raise ValueError(f"speaker id {speaker} out of range: the checkpoint has {config.num_speakers} speaker(s)")
     model = model_cls(config, None, train=False)                                         # :31

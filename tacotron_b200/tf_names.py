@@ -8,12 +8,18 @@ tensors keep their TF layouts (dense [in,out], conv [k,Cin,Cout], GRU gates/cand
 import re
 
 
-def tf_name_to_param(name, multi_speaker=False):
+def tf_name_to_param(name, multi_speaker=False, speaker_decoder=False):
     """TF-1.2-style variable name -> parameter name of tacotron_b200.params (same layouts, so a checkpoint tensor
     can be copied as is).  Raises KeyError for variables that are not part of the model (global_step, Adam slots,
     stft_mean/std, ...).  multi_speaker: the graph of a model with num_speakers > 1 (tacotron.py:116-124,
-    ops.py:101-115), whose encoder highway layers open with a speaker dense and a width-fixing dense."""
+    ops.py:101-115), whose encoder highway layers open with a speaker dense and a width-fixing dense.  speaker_decoder: the
+    speaker-conditioned decoder as well (Config.speaker_decoder): the dense of the reference's commented-out initial
+    attention line (`decoder/dense`, models/tacotron.py:96-97) and one dense per decoder GRU initial state."""
     import re
+    if speaker_decoder:
+        m = re.match(r"decoder/(?:speaker_state_([123])/)?dense/(kernel|bias)$", name)
+        if m:
+            return f"dec/spk/{'h' + m.group(1) if m.group(1) else 'attn'}/{'W' if m.group(2) == 'kernel' else 'b'}"
     if name == "embedding/embedding":
         return "embedding"
     if multi_speaker and name == "speaker/speaker_embed":

@@ -123,6 +123,9 @@ def main(argv=None):
     parser.add_argument("--summary-every", type=int, default=1, help="steps between two per-step summaries")
     parser.add_argument("--max-ctas", type=int, default=None,
                         help="CTAs (SMs) the decoder kernels may occupy, at least 32 (default: all the device holds)")
+    parser.add_argument("--speaker-decoder", action="store_true",
+                        help="multi-speaker data: condition the decoder on the speaker too (initial attention vector and "
+                             "GRU states)")
     args = parser.parse_args(argv)
     from .models.tacotron import Config, Tacotron
     config = Config()
@@ -130,6 +133,7 @@ def main(argv=None):
     config.restore = args.restore
     config.save_path = "debug" if args.debug else "%s/tacotron" % args.train_set         # :110-113
     config.max_ctas = args.max_ctas
+    config.speaker_decoder = args.speaker_decoder
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "train") if args.summaries else None     # train.py:41
     train(Tacotron, config, num_steps=args.steps, summary_dir=summary_dir, summary_every=args.summary_every)
