@@ -94,14 +94,23 @@ typedef struct taco_linear_desc {
 } taco_linear_desc;
 
 int taco_linear_fwd(const taco_linear_desc* d, void* stream);
+/* The launch taco_linear_fwd makes for descriptor d, decided on the host (no CUDA call, no device needed; pointers are
+ * only checked for alignment).  Returns taco_linear_fwd's error, with the same message, for a descriptor it rejects.
+ * Tensor-core impls: *bn = n-tile width (32: fp32x3 when at most 33 output tiles and N >= 64; 256: highway; else 128),
+ * *stages = k-block ring depth, *mode = 0 normal / 1 highway epilogue, *direct = 1 register-direct epilogue (every row
+ * segment it touches 16-byte aligned) / 0 transposing epilogue, *tile_stride = 128, or 127 with the fused max-pool.
+ * SIMT: 64 x 64 tiles over the flattened rows (*bn = 64, *stages = 1, *direct = 0, *tile_stride = 64).
+ * Any output pointer may be NULL.                                                                                */
+int taco_linear_route(const taco_linear_desc* d, int* bn, int* stages, int* mode, int* direct, int* tile_stride);
 
 /* Pack one TF-layout weight W[taps][C][N] into the tensor-core operand layout: row n of dst
  * (dst + (n)*ld_dst) holds, for tap j and channel c, W[j][c][n] at column j*round_up(C,32)+c,
- * rounded to TF32 (round-to-nearest); padding channels are zero.                             */
+ * rounded to TF32 (round-to-nearest, ties away from zero: cvt.rna); padding channels are zero.  */
 int taco_pack_weight(const float* W, int taps, int C, int N, float* dst, int64_t ld_dst, void* stream);
-/* 3xTF32 operand pair for TACO_IMPL_TC3: dst_hi rows = TF32 round-to-nearest heads, dst_lo rows = the remainders
- * (W - hi, cut to TF32); same layout as taco_pack_weight.  For a bank, call once per filter with the row offsets
- * of that filter in the hi half and in the lo half (lo half starts at row bank_K*bank_cout).                 */
+/* 3xTF32 operand pair for TACO_IMPL_TC3: dst_hi rows = TF32 round-to-nearest heads (ties away from zero), dst_lo rows =
+ * the remainders W - hi rounded to the nearest TF32 value (ties away from zero), so |hi + lo - W| <= 2^-22 |W|; same
+ * layout as taco_pack_weight.  For a bank, call once per filter with the row offsets of that filter in the hi half
+ * and in the lo half (lo half starts at row bank_K*bank_cout).                                                    */
 int taco_pack_weight_x3(const float* W, int taps, int C, int N, float* dst_hi, float* dst_lo, int64_t ld_dst, void* stream);
 
 /* tf.layers.max_pooling1d(pool 2, stride 1, 'same') over t  (models/ops.py:66-71)            */

@@ -95,7 +95,8 @@ _lib = None
 
 # every symbol include/taco_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
-    "taco_last_error", "taco_version", "taco_device_info", "taco_linear_fwd", "taco_pack_weight", "taco_pack_weight_x3",
+    "taco_last_error", "taco_version", "taco_device_info", "taco_linear_fwd", "taco_linear_route", "taco_pack_weight",
+    "taco_pack_weight_x3",
     "taco_maxpool_fwd", "taco_gather_rows", "taco_mask_rows", "taco_bigru_fwd", "taco_bigru_fwd_h0",
     "taco_decoder_packed_bytes", "taco_decoder_workspace_bytes", "taco_decoder_pack", "taco_decoder_fwd",
     "taco_decoder_capacity",
@@ -130,6 +131,7 @@ def lib():
     L.taco_version.restype = C.c_int
     L.taco_device_info.argtypes = [C.POINTER(C.c_int)] * 3
     L.taco_linear_fwd.argtypes = [C.POINTER(LinearDesc), C.c_void_p]
+    L.taco_linear_route.argtypes = [C.POINTER(LinearDesc)] + [C.POINTER(C.c_int)] * 5
     L.taco_pack_weight.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
     L.taco_conv_dw.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64] + [C.c_int32] * 6 + [C.c_void_p]
     L.taco_pack_weight_x3.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
@@ -195,6 +197,13 @@ def check(rc, what=""):
     if rc != 0:
         msg = lib().taco_last_error().decode("utf-8", "replace")
         raise TacoError(f"{what} failed (rc={rc}): {msg}")
+
+
+def linear_route(d):
+    """(bn, stages, mode, direct, tile_stride) of the launch taco_linear_fwd makes for LinearDesc d (host only)."""
+    out = [C.c_int() for _ in range(5)]
+    check(lib().taco_linear_route(C.byref(d), *[C.byref(v) for v in out]), "taco_linear_route")
+    return tuple(v.value for v in out)
 
 
 def ptr(t):

@@ -15,6 +15,7 @@ void taco_set_error(const char* fmt, ...) {
 
 int taco_linear_simt(const taco_linear_desc* d, cudaStream_t st);
 int taco_linear_tc(const taco_linear_desc* d, cudaStream_t st);
+int taco_linear_tc_route(const taco_linear_desc* d, TcRoute* r);
 int taco_pack_weight_impl(const float* W, int taps, int C, int N, float* dst, int64_t ld_dst, cudaStream_t st);
 int taco_pack_weight_x3_impl(const float* W, int taps, int C, int N, float* dst_hi, float* dst_lo, int64_t ld_dst, cudaStream_t st);
 int taco_conv_dw_tc_impl(float* dW, int64_t ldw, int64_t tap_stride, const float* X, int64_t ldx, const float* dZ, int64_t lddz,
@@ -99,6 +100,26 @@ __global__ void l1_stage2(const float* __restrict__ partial, int n, float* __res
     }
 }
 
+// the checks every taco_linear_fwd descriptor passes, whichever kernel runs it
+int linear_check(const taco_linear_desc* d) {
+    TACO_CHECK(d != nullptr, "taco_linear_fwd: NULL descriptor");
+    TACO_CHECK(d->X && d->Y, "taco_linear_fwd: X or Y is NULL");
+    TACO_CHECK(d->B >= 0 && d->T >= 0 && d->C > 0 && d->N > 0, "taco_linear_fwd: bad sizes B=%d T=%d C=%d N=%d", d->B, d->T, d->C, d->N);
+    TACO_CHECK(d->bank_K > 0 || d->taps >= 1, "taco_linear_fwd: taps must be >= 1");
+    TACO_CHECK(d->ldx >= d->C, "taco_linear_fwd: ldx < C");
+    const bool highway = d->epilogue == TACO_EPI_HIGHWAY;
+    const int nout = highway ? d->N / 2 : d->N;
+    TACO_CHECK(d->ldy >= nout, "taco_linear_fwd: ldy %lld < %d output columns (N, or N/2 for highway)", (long long)d->ldy, nout);
+    TACO_CHECK(!d->residual || d->ldr >= d->N, "taco_linear_fwd: ldr %lld < N %d", (long long)d->ldr, d->N);
+    TACO_CHECK(!highway || !d->hx || d->ldhx >= nout, "taco_linear_fwd: ldhx %lld < U %d", (long long)d->ldhx, nout);
+    // both highway epilogues compute relu(H)*sig(T) + hx*(1-sig(T)) and nothing else: refuse fields they would ignore
+    TACO_CHECK(!highway || (d->act == TACO_ACT_NONE && !d->scale && !d->shift && !d->keep && !d->residual && !d->pool),
+               "taco_linear_fwd: the highway epilogue takes only bias and hx (act, scale, shift, keep, residual, pool are not applied)");
+    TACO_CHECK(!d->bias_utt || (!highway && d->ldbu >= d->N),
+               "taco_linear_fwd: bias_utt needs the normal epilogue and ldbu >= N");
+    return 0;
+}
+
 inline int grid_for(int64_t total, int block) {
     int64_t g = (total + block - 1) / block;
     if (g > TACO_SMS * 16) g = TACO_SMS * 16;
@@ -125,17 +146,32 @@ int taco_device_info(int* sm_count, int* cc_major, int* cc_minor) {
 }
 
 int taco_linear_fwd(const taco_linear_desc* d, void* stream) {
-    TACO_CHECK(d != nullptr, "taco_linear_fwd: NULL descriptor");
-    TACO_CHECK(d->X && d->Y, "taco_linear_fwd: X or Y is NULL");
-    TACO_CHECK(d->B >= 0 && d->T >= 0 && d->C > 0 && d->N > 0, "taco_linear_fwd: bad sizes B=%d T=%d C=%d N=%d", d->B, d->T, d->C, d->N);
-    TACO_CHECK(d->bank_K > 0 || d->taps >= 1, "taco_linear_fwd: taps must be >= 1");
-    TACO_CHECK(d->ldx >= d->C, "taco_linear_fwd: ldx < C");
-    TACO_CHECK(!d->bias_utt || (d->epilogue != TACO_EPI_HIGHWAY && d->ldbu >= d->N),
-               "taco_linear_fwd: bias_utt needs the normal epilogue and ldbu >= N");
+    if (int rc = linear_check(d)) return rc;
     if (d->impl == TACO_IMPL_SIMT) return taco_linear_simt(d, (cudaStream_t)stream);
     if (d->impl == TACO_IMPL_TC || d->impl == TACO_IMPL_TC3) return taco_linear_tc(d, (cudaStream_t)stream);
     taco_set_error("taco_linear_fwd: unknown impl %d", d->impl);
     return 1;
+}
+
+int taco_linear_route(const taco_linear_desc* d, int* bn, int* stages, int* mode, int* direct, int* tile_stride) {
+    if (int rc = linear_check(d)) return rc;
+    TcRoute r;
+    if (d->impl == TACO_IMPL_SIMT) {
+        // gemm_simt.cu: 64 x 64 tiles over the flattened rows, one k-block in shared memory, element-wise epilogue
+        TACO_CHECK(!d->pool, "taco_linear_fwd(SIMT): fused max-pool is only available on the tensor-core path");
+        r.bn = 64; r.stages = 1; r.mode = d->epilogue == TACO_EPI_HIGHWAY ? 1 : 0; r.direct = 0; r.tile_stride = 64;
+    } else if (d->impl == TACO_IMPL_TC || d->impl == TACO_IMPL_TC3) {
+        if (int rc = taco_linear_tc_route(d, &r)) return rc;
+    } else {
+        taco_set_error("taco_linear_fwd: unknown impl %d", d->impl);
+        return 1;
+    }
+    if (bn) *bn = r.bn;
+    if (stages) *stages = r.stages;
+    if (mode) *mode = r.mode;
+    if (direct) *direct = r.direct;
+    if (tile_stride) *tile_stride = r.tile_stride;
+    return 0;
 }
 
 int taco_pack_weight_x3(const float* W, int taps, int C, int N, float* dst_hi, float* dst_lo, int64_t ld_dst, void* stream) {

@@ -55,6 +55,15 @@ extern unsigned long long g_taco_launches;   // kernels launched by this library
 
 static inline bool taco_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// launch route of a tensor-core taco_linear_fwd (gemm_tc.cu taco_linear_tc_route; reported by taco_linear_route)
+struct TcRoute {
+    int bn;            // n-tile width: 32, 128 or 256 (highway)
+    int stages;        // k-block ring depth
+    int mode;          // 0 normal epilogue, 1 highway
+    int direct;        // 1 register-direct epilogue, 0 transposing epilogue
+    int tile_stride;   // rows between consecutive m-tiles of an utterance: 128, or 127 with the fused max-pool
+};
+
 // SMs of the H100 SXM: sizes grid-stride launches and the split-K of the weight-gradient kernel
 constexpr int TACO_SMS = 132;
 
@@ -62,11 +71,13 @@ constexpr int TACO_SMS = 132;
 // device math
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float sigmoidf_acc(float x) {
-    // 1/(1+exp(-x)) with the fast exp2 path (rel. err ~1e-7 after the division)
+    // 1/(1+exp(-x)) with the fast exp2 path (rel. err ~1e-7 after the division; abs err <= 2.5e-7 for any finite x:
+    // __expf's error grows with |x| only where sigmoid'(x) is small, and __fdividef adds 2 ulp)
     return __fdividef(1.0f, 1.0f + __expf(-x));
 }
 __device__ __forceinline__ float tanhf_acc(float x) {
-    // tanh(x) = 1 - 2/(exp(2x)+1); exact limits at +-inf, abs err ~2e-7
+    // tanh(x) = 1 - 2/(exp(2x)+1); exact limits at +-inf, abs err ~2e-7 (<= 5e-7: 2 ulp of the quotient in [1, 2) for
+    // x < 0, plus __expf's error)
     float e = __expf(2.0f * x);
     return 1.0f - __fdividef(2.0f, e + 1.0f);
 }

@@ -313,6 +313,9 @@ __global__ void __launch_bounds__(TC_THREADS, MODE == 1 ? 1 : 2) gemm_tc_kernel(
                         if (row_ok) {
 #pragma unroll
                             for (int h = 0; h < 2; ++h) {
+                                // N % 16 == 0 here: a 16-column half is either all inside the row or all past its end
+                                // (the next row's mask, or past the buffer on the last row) and then not loaded
+                                if (n0 + c0 + 16 * h >= a.e.N) break;
                                 const uint4 kk = kp[h];
                                 const uint32_t ks[4] = {kk.x, kk.y, kk.z, kk.w};
 #pragma unroll
@@ -464,8 +467,9 @@ __global__ void pack_weight_kernel(const float* __restrict__ W, int taps, int C,
     }
 }
 
-// X3: hi = TF32 round-to-nearest head, lo = (W - hi) cut to TF32 (the remainder has <= 13 significant bits; the cut drops
-// at most 2^-22 |W|) -- both exactly representable, so the tensor core's own fp32 -> tf32 narrowing cannot change them
+// X3: hi = TF32 round-to-nearest head (ties away from zero), lo = (W - hi) rounded to the nearest TF32 value (ties away
+// from zero; W - hi is exact and has at most 13 significant bits, so the rounding drops at most 2^-22 |W|) -- both
+// exactly representable, so the tensor core's own fp32 -> tf32 narrowing cannot change them
 __global__ void pack_weight_x3_kernel(const float* __restrict__ W, int taps, int C, int N, int Cpad,
                                       float* __restrict__ dst_hi, float* __restrict__ dst_lo, int64_t ld) {
     int64_t total = (int64_t)N * taps * Cpad;
@@ -765,21 +769,56 @@ int taco_conv_dw_tc_impl(float* dW, int64_t ldw, int64_t tap_stride, const float
     return 0;
 }
 
-int taco_linear_tc(const taco_linear_desc* d, cudaStream_t st) {
+// The dispatch decision of taco_linear_tc, host only (no CUDA call): every check of a tensor-core descriptor that needs no
+// device, then which kernel instantiation and which epilogue the launch uses.
+int taco_linear_tc_route(const taco_linear_desc* d, TcRoute* r) {
     TACO_CHECK(d->Wp != nullptr, "taco_linear_fwd(TC): Wp (packed weights) is NULL");
     TACO_CHECK(taco_aligned16(d->X) && taco_aligned16(d->Wp), "taco_linear_fwd(TC): X / Wp must be 16-byte aligned");
     TACO_CHECK((d->ldx % 4) == 0 && (d->ldwp % 4) == 0, "taco_linear_fwd(TC): ldx and ldwp must be multiples of 4 floats (TMA 16B strides)");
+    const bool highway = d->epilogue == TACO_EPI_HIGHWAY;
+    if (highway) TACO_CHECK(d->N == 256 && d->taps == 1 && d->bank_K == 0 && d->hx, "highway (TC): needs N == 256 (U = 128), dense, hx");
+    if (d->bank_K > 0) TACO_CHECK(d->bank_cout == 128 && d->N == d->bank_K * 128, "bank (TC): bank_cout must be 128");
+    if (d->pool) TACO_CHECK(!highway && !d->residual && !d->keep, "pool cannot be combined with highway / residual / dropout");
+    const int Cpad = (d->C + 31) / 32 * 32;
+    const int max_taps = d->bank_K > 0 ? d->bank_K : d->taps;
+    TACO_CHECK(d->ldwp >= (int64_t)max_taps * Cpad, "taco_linear_fwd(TC): ldwp too small for taps*Cpad");
+
+    const bool x3 = d->impl == TACO_IMPL_TC3;
+    r->mode = highway ? 1 : 0;
+    r->bn = highway ? 256 : 128;
+    // few output tiles (encoder-side contractions: 32 utterances x 128 characters = 32 m-tiles): 32-column n-tiles put
+    // four times as many CTAs on the machine, each with a 6-deep ring (with 128-column tiles the long-K conv projection
+    // 2048x3 -> 128 would run on 32 of the 132 SMs)
+    {
+        const int64_t mt = (int64_t)((d->T + TC_BM - 1) / TC_BM) * d->B;
+        if (x3 && !highway && d->bank_K == 0 && !d->pool && mt * ((d->N + 127) / 128) <= TACO_SMS / 4 && d->N >= 64) r->bn = 32;
+    }
+    if (x3) r->stages = r->bn == 32 ? 6 : 2;
+    // tf32: short K loops (<= 8 k-iterations: dense 128/256-wide inputs) are epilogue/latency bound: a 2-stage ring suffices
+    else r->stages = (highway || (d->bank_K == 0 && d->taps * (Cpad / 32) <= 8)) ? 2 : 3;
+    // register-direct epilogue: needs 16-byte aligned row segments everywhere it touches
+    {
+        const int nout = highway ? d->N / 2 : d->N;
+        bool ok = (d->ldy % 4) == 0 && (nout % 4) == 0 && taco_aligned16(d->Y);
+        if (d->residual) ok = ok && (d->ldr % 4) == 0 && taco_aligned16(d->residual);
+        if (d->hx) ok = ok && (d->ldhx % 4) == 0 && taco_aligned16(d->hx);
+        if (d->keep) ok = ok && (nout % 16) == 0 && taco_aligned16(d->keep);
+        r->direct = ok ? 1 : 0;
+    }
+    r->tile_stride = d->pool ? (TC_BM - 1) : TC_BM;
+    return 0;
+}
+
+int taco_linear_tc(const taco_linear_desc* d, cudaStream_t st) {
+    TcRoute r;
+    if (int rc = taco_linear_tc_route(d, &r)) return rc;
     EncodeTiledFn enc = get_encode_fn();
     TACO_CHECK(enc != nullptr, "cuTensorMapEncodeTiled driver entry point not available");
     const int64_t M = (int64_t)d->B * d->T;
     if (M == 0 || d->N == 0) return 0;
 
-    const bool highway = d->epilogue == TACO_EPI_HIGHWAY;
-    int BN = highway ? 256 : 128;
-    if (highway) TACO_CHECK(d->N == 256 && d->taps == 1 && d->bank_K == 0 && d->hx, "highway (TC): needs N == 256 (U = 128), dense, hx");
-    if (d->bank_K > 0) TACO_CHECK(d->bank_cout == 128 && d->N == d->bank_K * 128, "bank (TC): bank_cout must be 128");
-    if (d->pool) TACO_CHECK(!highway && !d->residual && !d->keep, "pool cannot be combined with highway / residual / dropout");
-
+    const bool highway = r.mode == 1;
+    const int BN = r.bn;
     TcArgs a;
     a.B = d->B; a.T = d->T;
     a.Cpad = (d->C + 31) / 32 * 32;
@@ -788,33 +827,15 @@ int taco_linear_tc(const taco_linear_desc* d, cudaStream_t st) {
     a.N = d->N;
     a.pool = d->pool ? 1 : 0;
     const bool x3 = d->impl == TACO_IMPL_TC3;
-    // few output tiles (encoder-side contractions: 32 utterances x 128 characters = 32 m-tiles): 32-column n-tiles put
-    // four times as many CTAs on the machine, each with a 6-deep ring (with 128-column tiles the long-K conv projection
-    // 2048x3 -> 128 would run on 32 of the 132 SMs)
-    {
-        const int64_t mt = (int64_t)((d->T + TC_BM - 1) / TC_BM) * d->B;
-        if (x3 && !highway && d->bank_K == 0 && !d->pool && mt * ((d->N + 127) / 128) <= TACO_SMS / 4 && d->N >= 64) BN = 32;
-    }
-    // register-direct epilogue: needs 16-byte aligned row segments everywhere it touches
-    {
-        const int nout = highway ? d->N / 2 : d->N;
-        bool ok = (d->ldy % 4) == 0 && (nout % 4) == 0 && taco_aligned16(d->Y);
-        if (d->residual) ok = ok && (d->ldr % 4) == 0 && taco_aligned16(d->residual);
-        if (d->hx) ok = ok && (d->ldhx % 4) == 0 && taco_aligned16(d->hx);
-        if (d->keep) ok = ok && (nout % 16) == 0 && taco_aligned16(d->keep);
-        a.direct = ok ? 1 : 0;
-    }
+    a.direct = r.direct;
     a.lo_row0 = d->N;                                    // packed buffer = [hi rows 0..N) | lo rows N..2N)
-    a.tile_stride = a.pool ? (TC_BM - 1) : TC_BM;
+    a.tile_stride = r.tile_stride;
     a.tiles_per_seq = a.pool ? ((d->T - 1 + a.tile_stride - 1) / a.tile_stride) : ((d->T + TC_BM - 1) / TC_BM);
     if (a.tiles_per_seq < 1) a.tiles_per_seq = 1;
     a.e.Y = d->Y; a.e.ldy = d->ldy; a.e.bias = d->bias; a.e.scale = d->scale; a.e.shift = d->shift;
     a.e.keep = d->keep; a.e.keep_scale = d->keep_scale; a.e.residual = d->residual; a.e.ldr = d->ldr;
     a.e.hx = d->hx; a.e.ldhx = d->ldhx; a.e.act = d->act; a.e.N = highway ? d->N / 2 : d->N;
     a.e.bias_utt = d->bias_utt; a.e.ldbu = d->ldbu; a.e.T = d->T;
-
-    const int max_taps = d->bank_K > 0 ? d->bank_K : d->taps;
-    TACO_CHECK(d->ldwp >= (int64_t)max_taps * a.Cpad, "taco_linear_fwd(TC): ldwp too small for taps*Cpad");
 
     CUtensorMap tmA, tmB;
     {
@@ -846,7 +867,6 @@ int taco_linear_tc(const taco_linear_desc* d, cudaStream_t st) {
         return launch_tc<128, 2, 0, true>(tmA, tmB, a, grid, st);
     }
     if (highway) return launch_tc<256, 2, 1>(tmA, tmB, a, grid, st);
-    // short K loops (<= 8 k-iterations: dense 128/256-wide inputs) are epilogue/latency bound: a 2-stage ring suffices
-    if (!a.bank && a.taps * a.cchunks <= 8) return launch_tc<128, 2, 0>(tmA, tmB, a, grid, st);
+    if (r.stages == 2) return launch_tc<128, 2, 0>(tmA, tmB, a, grid, st);
     return launch_tc<128, 3, 0>(tmA, tmB, a, grid, st);
 }
