@@ -350,6 +350,37 @@ int taco_gl_phase(float* full_c64, const float* mag, const float* rebuilt_c64, i
  * radix-2 Stockham transform, one CTA per row: no FFT library on the path.                                          */
 int taco_rfft2048(float* X_c64, const float* x, int64_t rows, void* stream);
 int taco_irfft2048(float* x, const float* X_c64, int64_t rows, void* stream);
+/* Where each utterance's speech ends, for the opt-in tail trim of synthesis (tacotron_b200.audio.speech_frames).  The
+ * training targets end in padding frames of log(0 + 1e-8) (preprocessing zero-pads the trimmed waveform,
+ * features.cu feature_spec), so a trained model ends each utterance with frames far below its speech.
+ * spec [B][T][F*r] is the post-net output in the decoder's layout, scale/shift [F*r] the optional de-normalisation
+ * (both or neither, as in taco_gl_init).  Writes frames[b], the number of STFT frames to keep:
+ *   - frame space is the one gl_init uses: n = 4r*(T/4) frames, frame f = 4r*q + 4c + l comes from decoder step
+ *     t = 4q + l, column block c (reshape_frames(forward=False), audio.py:30-35);
+ *   - log magnitude v[f,k] = spec[b, t, c*F + k]*scale + shift, as in gl_init;
+ *   - log power e[f] = log sum_k exp(2 v[f,k]), a max-shifted float32 sum in a fixed reduction order;
+ *   - E = max_f e[f]; frame f is voiced when e[f] >= E - top_db*ln(10)/10;
+ *   - f* = the last voiced frame; frames[b] = 4r * clamp(ceil((f*+1) / 4r), k_min, T/4), k_min = ceil(5 / 4r)
+ *     (the inversion's reflect padding needs at least 5 frames: hop*(n-1) > n_fft/2);
+ *   - frames[b] = n when any e[f] or E is not finite.
+ * Whole blocks of 4r frames are the outputs of decoder steps [0, frames[b]/r).  Two launches (one warp per frame, then
+ * one CTA per utterance) and a stream-ordered scratch of B*n floats; no host synchronisation.
+ * B >= 1, r >= 1, T >= 4, F >= 1, top_db finite and > 0.  Semantics: tests/mirror_kernels_trim.py speech_frames.     */
+int taco_speech_frames(int* frames, const float* spec, int B, int T, int r, int F, const float* scale, const float* shift,
+                       float top_db, void* stream);
+/* Griffin-Lim over a packed batch (tacotron_b200.audio.invert_speech): utterance b owns rows [off[b], off[b+1]) of
+ * mag / full / phase_u [N][F] and of the frame buffer [N][n_fft] (off int64 [B+1], off[0] = 0, N = off[B]), and its
+ * L_b = hop*(n_b - 1) samples start at hop*(off[b] - b) of one flat y.  The per-element arithmetic is that of
+ * taco_gl_init / taco_gl_ola / taco_gl_frame, so utterance b is bit-identical to those run on it alone; gl_ola clamps
+ * its frames to n_b - 1 and gl_frame reflects at L_b.  One launch over the whole batch each (blockIdx.y = utterance);
+ * max_frames (the largest n_b) sizes the grid.  Each n_b must lie in [5, 4r*(T/4)] (gl_init reads spec[b, :T]).
+ * taco_rfft2048 / taco_irfft2048 / taco_gl_phase run unchanged on the N rows.  Semantics: tests/mirror_kernels_trim.py. */
+int taco_gl_init_packed(float* full_c64, float* mag, const float* spec, const float* phase_u, const int64_t* off,
+                        int B, int T, int r, int F, int max_frames, const float* scale, const float* shift, void* stream);
+int taco_gl_ola_packed(float* y, const float* fr, const int64_t* off, int B, int max_frames, int hop, int n_fft,
+                       int win_length, void* stream);
+int taco_gl_frame_packed(float* frw, const float* y, const int64_t* off, int B, int max_frames, int hop, int n_fft,
+                         int win_length, void* stream);
 
 /* Input data format (SURVEY 8(f) rank 3): spectrograms are stored float16 (preprocess.py:179-180) and normalised in
  * that dtype (data_input.py:56-64) before the float32 cast (:38-39).  Bit-exact device version of those statements:

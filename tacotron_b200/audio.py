@@ -14,6 +14,8 @@ round 1 called cuFFT through ``torch.fft`` here); everything between them is fou
 so one iteration is irfft2048 -> gl_ola -> gl_frame -> rfft2048 -> gl_phase: 5 launches of this library, ~20 MB of HBM traffic per utterance of
 500 frames.  All arithmetic goes through the kernel namespace K (tacotron_b200/kernels.py); tests run the same
 orchestration over tests/mirror_kernels.py on CPU tensors against the numpy oracle (oracle/audio_oracle.py).
+``speech_frames`` / ``invert_speech`` are the opt-in tail trim of synthesis: where each utterance's speech ends
+(taco_speech_frames), then the same loop over only the kept frames of the batch, packed end to end.
 
 Feature extraction (the reference's ``process_audio``, audio.py:38-65, used by tacotron_b200/preprocess.py) is the
 analysis half of the same transform: trim_bounds -> feature_frames -> rfft2048 -> feature_spec, four launches per chunk of
@@ -334,19 +336,78 @@ def griffinlim_batch(spec, r, n_iter=50, scale=None, shift=None, phase_u=None, K
     return y
 
 
-def _gl_iterations(K, full, mag, spec, phase_u, r, scale, shift, y, frw, n_iter, rebuilt=None):
-    """frw [B, n, 2048] doubles as the istft frame buffer: irfft writes it, gl_ola consumes it, gl_frame refills it."""
+def _gl_iterations(K, full, mag, spec, phase_u, r, scale, shift, y, frw, n_iter, rebuilt=None, packed=None):
+    """frw [B, n, 2048] doubles as the istft frame buffer: irfft writes it, gl_ola consumes it, gl_frame refills it.
+    packed: (off, max_frames) of invert_speech's packed layout (rows off[b]:off[b+1] per utterance), None for [B, n, .]."""
     if rebuilt is None:
         rebuilt = torch.empty_like(full)
-    K.gl_init(full, mag, spec, phase_u, r, scale, shift)
+    if packed is None:
+        K.gl_init(full, mag, spec, phase_u, r, scale, shift)
+        ola = functools.partial(K.gl_ola, y, frw, hop_length, win_length)
+        frame = functools.partial(K.gl_frame, frw, y, hop_length, win_length)
+    else:
+        off, nmax = packed
+        K.gl_init_packed(full, mag, spec, phase_u, off, r, nmax, scale, shift)
+        ola = functools.partial(K.gl_ola_packed, y, frw, off, nmax, hop_length, win_length)
+        frame = functools.partial(K.gl_frame_packed, frw, y, off, nmax, hop_length, win_length)
     for it in range(n_iter + 1):
         K.irfft2048(frw, full)                                               # inverse real FFT of every frame
-        K.gl_ola(y, frw, hop_length, win_length)
+        ola()
         if it == n_iter:
             break
-        K.gl_frame(frw, y, hop_length, win_length)
+        frame()
         K.rfft2048(rebuilt, frw)                                             # real FFT of every re-framed, windowed frame
         K.gl_phase(full, mag, rebuilt)
+
+
+def speech_frames(spec, r, stft_mean=None, stft_std=None, top_db=TRIM_TOP_DB, K=None):
+    """STFT frames to keep of each utterance of spec [B, T, 1025*r] (the post-net output, de-normalised with stft_std /
+    stft_mean like invert_spectrogram) -> int32 [B] on spec's device, without a host synchronisation.  A frame is speech
+    when its power is within top_db of the utterance's loudest frame; frames[b] is the end of the last one, rounded up to
+    whole blocks of 4r frames (decoder steps [0, frames[b]/r)), at least 5 frames, and all 4r*(T//4) frames when the
+    spectrogram is not finite.  The training targets end in log(1e-8) padding frames, so a trained model is taught to go
+    quiet after its speech; the rule is reasoned from that, not observed on a trained model's output."""
+    K = K or _K()
+    scale, shift = (stft_std, stft_mean) if stft_std is not None else (None, None)
+    frames = torch.empty(spec.shape[0], dtype=torch.int32, device=spec.device)
+    K.speech_frames(frames, spec.contiguous(), r, scale, shift, top_db)
+    return frames
+
+
+def invert_speech(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, generator=None):
+    """invert_spectrogram on the first frames[b] STFT frames of each utterance only (frames: speech_frames or the
+    caller's, a multiple of 4r in [5, 4r*(T//4)] each) -> list of B 1-D waveforms of hop*(frames[b]-1) samples.  The kept
+    frames are packed end to end, so one iteration is still 5 launches; utterance b equals invert_spectrogram on
+    spec[b:b+1, :frames[b]//r] with the same initial phases.  phase_u: packed uniform [0,1) phases [sum(frames), 1025],
+    drawn on the device if None.  Reads frames to the host once."""
+    K = K or _K()
+    B, T, W = spec.shape
+    assert W == F_BINS * r, (W, r)
+    n = 4 * r * (T // 4)
+    fr = np.asarray(frames.cpu() if torch.is_tensor(frames) else frames).astype(np.int64).reshape(-1)
+    if fr.shape != (B,):
+        raise ValueError(f"invert_speech: {fr.size} frame counts for {B} utterances")
+    bad = np.flatnonzero((fr % (4 * r) != 0) | (fr < 5) | (fr > n))
+    if bad.size:
+        b = int(bad[0])
+        raise ValueError(f"invert_speech: frames[{b}] = {int(fr[b])} must be a multiple of 4r = {4 * r} in [5, {n}]")
+    off = np.zeros(B + 1, dtype=np.int64)
+    np.cumsum(fr, out=off[1:])
+    N, nmax = int(off[-1]), int(fr.max())
+    rdt, dev = spec.dtype, spec.device
+    cdt = torch.complex64 if rdt == torch.float32 else torch.complex128
+    if phase_u is None:
+        phase_u = torch.rand((N, F_BINS), dtype=rdt, device=dev, generator=generator)
+    elif phase_u.shape != (N, F_BINS):
+        raise ValueError(f"invert_speech: phase_u must be the packed [{N}, {F_BINS}], got {tuple(phase_u.shape)}")
+    scale, shift = (stft_std, stft_mean) if stft_std is not None else (None, None)
+    mag = torch.empty((N, F_BINS), dtype=rdt, device=dev)
+    full = torch.empty((N, F_BINS), dtype=cdt, device=dev)
+    y = torch.empty(hop_length * (N - B), dtype=rdt, device=dev)
+    frw = torch.empty((N, n_fft), dtype=rdt, device=dev)
+    _gl_iterations(K, full, mag, spec.contiguous(), phase_u.contiguous(), r, scale, shift, y, frw, n_iter,
+                   packed=(torch.from_numpy(off).to(dev), nmax))
+    return [y[hop_length * (off[b] - b):hop_length * (off[b + 1] - b - 1)] for b in range(B)]
 
 
 class GriffinLimGraph:

@@ -18,14 +18,29 @@ inline int grid_for(int64_t total, int block) {
     return (int)g;
 }
 
+// The three kernels below that need to know which utterance an element belongs to take `off`:
+//   off == nullptr: the padded layout, utterance b = rows [b*n, (b+1)*n), samples [b*L, (b+1)*L); a 1-D grid-stride loop
+//                   over every element of the batch.
+//   off != nullptr: the packed layout of taco_*_packed, utterance b = blockIdx.y = rows [off[b], off[b+1]) (n_b of them)
+//                   and L_b = hop*(n_b - 1) samples from hop*(off[b] - b); the grid-stride loop runs over that
+//                   utterance's elements only.
+// The per-element arithmetic is the same code in both layouts, so a packed utterance is bit-identical to the padded
+// path run on it alone.
+
 // mag[b,f,k] = exp(spec[b, t(f), c(f)*F + k] * scale + shift);  full = mag * exp(2 pi i u)
 __global__ void gl_init_kernel(float2* __restrict__ full, float* __restrict__ mag, const float* __restrict__ spec,
                                const float* __restrict__ phase_u, int T, int n, int r, int F, const float* __restrict__ scale,
-                               const float* __restrict__ shift, int64_t total) {
+                               const float* __restrict__ shift, const int64_t* __restrict__ off, int64_t total) {
+    int64_t base = 0;                                                   // first output element of this utterance
+    if (off) {
+        base = off[blockIdx.y] * F;
+        total = (off[blockIdx.y + 1] - off[blockIdx.y]) * F;
+    }
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int k = (int)(i % F);
-        const int f = (int)((i / F) % n);
-        const int b = (int)(i / ((int64_t)F * n));
+        const int f = off ? (int)(i / F) : (int)((i / F) % n);
+        const int b = off ? (int)blockIdx.y : (int)(i / ((int64_t)F * n));
+        const int64_t o = base + i;
         const int b4 = f / (4 * r), rem = f % (4 * r);
         const int c = rem >> 2, tl = rem & 3;
         const int t = 4 * b4 + tl;
@@ -34,19 +49,28 @@ __global__ void gl_init_kernel(float2* __restrict__ full, float* __restrict__ ma
         if (scale) v = fmaf(v, scale[col], shift[col]);
         const float m = expf(v);
         float s, co;
-        sincospif(2.0f * phase_u[i], &s, &co);
-        mag[i] = m;
-        full[i] = make_float2(m * co, m * s);
+        sincospif(2.0f * phase_u[o], &s, &co);
+        mag[o] = m;
+        full[o] = make_float2(m * co, m * s);
     }
 }
 
 // y[b,s] = sum_t w[j] fr[b,t,j] / sum_t w[j]^2,  j = s + n_fft/2 - t*hop inside the window support
 __global__ void gl_ola_kernel(float* __restrict__ y, const float* __restrict__ fr, int n, int L, int hop, int n_fft, int win_length,
-                              int64_t total) {
+                              const int64_t* __restrict__ off, int64_t total) {
     const int lpad = (n_fft - win_length) / 2;
+    int64_t row0 = 0, ybase = 0;
+    if (off) {
+        row0 = off[blockIdx.y];
+        n = (int)(off[blockIdx.y + 1] - row0);
+        L = hop * (n - 1);
+        ybase = (int64_t)hop * (row0 - blockIdx.y);
+        total = n >= 2 ? L : 0;
+    }
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int s = (int)(i % L);
         const int b = (int)(i / L);
+        const int64_t frow = off ? row0 : (int64_t)b * n;
         const int p = s + n_fft / 2;
         // frames whose window support [t*hop + lpad, t*hop + lpad + win_length) contains p
         int tmax = (p - lpad) / hop;
@@ -57,17 +81,26 @@ __global__ void gl_ola_kernel(float* __restrict__ y, const float* __restrict__ f
         for (int t = tmin; t <= tmax; ++t) {
             const int j = p - t * hop;
             const float w = hann_at(j, lpad, win_length);
-            acc = fmaf(w, fr[((int64_t)b * n + t) * n_fft + j], acc);
+            acc = fmaf(w, fr[(frow + t) * n_fft + j], acc);
             ss = fmaf(w, w, ss);
         }
-        y[i] = (ss > FLT_MIN) ? acc / ss : acc;
+        y[ybase + i] = (ss > FLT_MIN) ? acc / ss : acc;
     }
 }
 
 // frw[b,t,j] = w[j] * ypad[t*hop + j],  ypad = y reflect-padded by n_fft/2 on both sides
 __global__ void gl_frame_kernel(float* __restrict__ frw, const float* __restrict__ y, int n, int L, int hop, int n_fft, int win_length,
-                                int64_t total) {
+                                const int64_t* __restrict__ off, int64_t total) {
     const int lpad = (n_fft - win_length) / 2;
+    int64_t base = 0, ybase = 0;
+    if (off) {
+        const int64_t row0 = off[blockIdx.y];
+        n = (int)(off[blockIdx.y + 1] - row0);
+        L = hop * (n - 1);
+        base = row0 * n_fft;
+        ybase = (int64_t)hop * (row0 - blockIdx.y);
+        total = L > n_fft / 2 ? (int64_t)n * n_fft : 0;             // the host rejects shorter ones; keep the reads in bounds
+    }
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int j = (int)(i % n_fft);
         const int t = (int)((i / n_fft) % n);
@@ -78,9 +111,9 @@ __global__ void gl_frame_kernel(float* __restrict__ frw, const float* __restrict
             int q = t * hop + j - n_fft / 2;
             if (q < 0) q = -q;
             if (q >= L) q = 2 * (L - 1) - q;
-            v = w * y[(int64_t)b * L + q];
+            v = w * y[ybase + (int64_t)b * L + q];
         }
-        frw[i] = v;
+        frw[base + i] = v;
     }
 }
 
@@ -91,6 +124,107 @@ __global__ void gl_phase_kernel(float2* __restrict__ full, const float* __restri
         const float a = hypotf(z.x, z.y);
         const float m = mag[i];
         full[i] = (a > 0.f) ? make_float2(m * (z.x / a), m * (z.y / a)) : make_float2(m, 0.f);
+    }
+}
+
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Where an utterance's speech ends (taco_speech_frames).  Two launches: frame_power_kernel spreads the read of the
+// spectrogram over the whole device, one warp per frame; speech_end_kernel then reduces each utterance's n powers with
+// one CTA.  Both reductions run in a fixed order, so the result does not change from run to run.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int SF_THREADS = 256;
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int m = 16; m > 0; m >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, m));
+    return v;
+}
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int m = 16; m > 0; m >>= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
+    return v;
+}
+
+// e[b*n + f] = log sum_k exp(2 v[f,k]),  v[f,k] = spec[b, t(f), c(f)*F + k] * scale + shift (gl_init's frame space),
+// as max-shifted sums: m = max_k 2v, e = m + log sum_k exp(2v - m).  NaN or +Inf in v, or a frame of -Inf only, makes
+// e non-finite.  Lane l sums bins l, l+32, ... in order, then the warp combines by butterfly.
+__global__ void __launch_bounds__(SF_THREADS) frame_power_kernel(float* __restrict__ e, const float* __restrict__ spec, int T,
+                                                                 int n, int r, int F, const float* __restrict__ scale,
+                                                                 const float* __restrict__ shift, int64_t frames) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (SF_THREADS / 32);
+    for (int64_t g = blockIdx.x * (int64_t)(SF_THREADS / 32) + threadIdx.x / 32; g < frames; g += warps) {
+        const int f = (int)(g % n);
+        const int64_t b = g / n;
+        const int b4 = f / (4 * r), rem = f % (4 * r);
+        const int c = rem >> 2, tl = rem & 3;
+        const int t = 4 * b4 + tl;
+        const float* row = spec + (b * T + t) * ((int64_t)F * r) + (int64_t)c * F;
+        const float* sc = scale ? scale + c * F : nullptr;
+        const float* sh = scale ? shift + c * F : nullptr;
+        float m = -INFINITY;
+        for (int k = lane; k < F; k += 32) {
+            float v = row[k];
+            if (sc) v = fmaf(v, sc[k], sh[k]);
+            m = fmaxf(m, 2.0f * v);
+        }
+        m = warp_max(m);
+        float s = 0.f;
+        for (int k = lane; k < F; k += 32) {
+            float v = row[k];
+            if (sc) v = fmaf(v, sc[k], sh[k]);
+            s += expf(2.0f * v - m);
+        }
+        s = warp_sum(s);
+        if (lane == 0) e[g] = m + logf(s);
+    }
+}
+
+// one CTA per utterance: E = max_f e[f]; f* = the last f with e[f] >= E - top_db ln(10)/10;
+// frames[b] = 4r * clamp(ceil((f* + 1) / 4r), ceil(5 / 4r), T/4), or n if any e[f] is not finite
+__global__ void __launch_bounds__(SF_THREADS) speech_end_kernel(int* __restrict__ frames, const float* __restrict__ e, int n, int r,
+                                                                int T, float top_db) {
+    __shared__ float rmax[SF_THREADS];
+    __shared__ int rlast[SF_THREADS];
+    const int tid = threadIdx.x;
+    const float* eb = e + (int64_t)blockIdx.x * n;
+    float m = -INFINITY;
+    int bad = 0;
+    for (int f = tid; f < n; f += SF_THREADS) {
+        const float x = eb[f];
+        if (fabsf(x) <= FLT_MAX) m = fmaxf(m, x);                    // finite (false for NaN and +-Inf)
+        else bad = 1;
+    }
+    rmax[tid] = m;
+    rlast[tid] = bad;
+    __syncthreads();
+    for (int s = SF_THREADS / 2; s > 0; s >>= 1) {
+        if (tid < s) {
+            rmax[tid] = fmaxf(rmax[tid], rmax[tid + s]);
+            rlast[tid] |= rlast[tid + s];
+        }
+        __syncthreads();
+    }
+    const float thr = rmax[0] - top_db * 0.230258509299404568f;       // ln(10) / 10: dB of power -> natural log
+    bad = rlast[0];
+    __syncthreads();
+    int last = -1;
+    for (int f = tid; f < n; f += SF_THREADS)
+        if (eb[f] >= thr) last = f;
+    rlast[tid] = last;
+    __syncthreads();
+    for (int s = SF_THREADS / 2; s > 0; s >>= 1) {
+        if (tid < s) rlast[tid] = max(rlast[tid], rlast[tid + s]);
+        __syncthreads();
+    }
+    if (tid == 0) {
+        const int blk = 4 * r;
+        int k = (rlast[0] + blk) / blk;                                 // ceil((f* + 1) / 4r)
+        const int kmin = (5 + blk - 1) / blk;                           // the inversion's reflect padding needs 5 frames
+        if (k < kmin) k = kmin;
+        if (k > T / 4) k = T / 4;
+        frames[blockIdx.x] = bad ? n : blk * k;
     }
 }
 
@@ -195,7 +329,7 @@ int taco_gl_init(float* full_c64, float* mag, const float* spec, const float* ph
     const int64_t total = (int64_t)B * n * F;
     if (total == 0) return 0;
     TACO_LAUNCH(gl_init_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, reinterpret_cast<float2*>(full_c64), mag, spec, phase_u, T, n, r, F,
-                                                                           scale, shift, total);
+                                                                           scale, shift, nullptr, total);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -206,7 +340,7 @@ int taco_gl_ola(float* y, const float* fr, int B, int n, int hop, int n_fft, int
     const int L = hop * (n - 1);
     const int64_t total = (int64_t)B * L;
     if (total == 0) return 0;
-    TACO_LAUNCH(gl_ola_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, y, fr, n, L, hop, n_fft, win_length, total);
+    TACO_LAUNCH(gl_ola_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, y, fr, n, L, hop, n_fft, win_length, nullptr, total);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -216,8 +350,81 @@ int taco_gl_frame(float* frw, const float* y, int B, int n, int hop, int n_fft, 
     const int L = hop * (n - 1);
     TACO_CHECK(n >= 2 && L > n_fft / 2, "taco_gl_frame: signal (%d samples) shorter than the reflect padding (%d)", L, n_fft / 2);
     const int64_t total = (int64_t)B * n * n_fft;
-    TACO_LAUNCH(gl_frame_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, frw, y, n, L, hop, n_fft, win_length, total);
+    TACO_LAUNCH(gl_frame_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, frw, y, n, L, hop, n_fft, win_length, nullptr, total);
     TACO_LAUNCH_CHECK();
+    return 0;
+}
+
+// grid of a packed launch: blockIdx.y = utterance, enough x-blocks for the longest one, the whole grid capped like grid_for
+static dim3 packed_grid(int64_t per_utt, int B) {
+    int64_t gx = (per_utt + 255) / 256;
+    const int64_t cap = TACO_SMS * 32 / B;
+    if (gx > cap) gx = cap;
+    if (gx < 1) gx = 1;
+    return dim3((unsigned)gx, (unsigned)B);
+}
+
+int taco_gl_init_packed(float* full_c64, float* mag, const float* spec, const float* phase_u, const int64_t* off, int B, int T,
+                        int r, int F, int max_frames, const float* scale, const float* shift, void* stream) {
+    TACO_CHECK(full_c64 && mag && spec && phase_u && off, "taco_gl_init_packed: NULL");
+    TACO_CHECK(B >= 1 && B <= 65535 && r >= 1 && T >= 4 && F >= 1, "taco_gl_init_packed: bad sizes (B=%d, T=%d, r=%d, F=%d)", B, T, r, F);
+    TACO_CHECK(max_frames >= 1 && max_frames <= 4 * r * (T / 4), "taco_gl_init_packed: max_frames=%d outside [1, 4*r*(T/4)]", max_frames);
+    TACO_CHECK((scale == nullptr) == (shift == nullptr), "taco_gl_init_packed: scale and shift go together");
+    TACO_LAUNCH(gl_init_kernel, packed_grid((int64_t)max_frames * F, B), 256, 0, (cudaStream_t)stream, reinterpret_cast<float2*>(full_c64),
+                mag, spec, phase_u, T, 4 * r * (T / 4), r, F, scale, shift, off, (int64_t)0);
+    TACO_LAUNCH_CHECK();
+    return 0;
+}
+
+int taco_gl_ola_packed(float* y, const float* fr, const int64_t* off, int B, int max_frames, int hop, int n_fft, int win_length,
+                       void* stream) {
+    TACO_CHECK(y && fr && off, "taco_gl_ola_packed: NULL");
+    TACO_CHECK(B >= 1 && B <= 65535 && max_frames >= 2 && hop >= 1 && win_length >= 1 && win_length <= n_fft,
+               "taco_gl_ola_packed: bad sizes");
+    TACO_LAUNCH(gl_ola_kernel, packed_grid((int64_t)hop * (max_frames - 1), B), 256, 0, (cudaStream_t)stream, y, fr, 0, 0, hop, n_fft,
+                win_length, off, (int64_t)0);
+    TACO_LAUNCH_CHECK();
+    return 0;
+}
+
+int taco_gl_frame_packed(float* frw, const float* y, const int64_t* off, int B, int max_frames, int hop, int n_fft, int win_length,
+                         void* stream) {
+    TACO_CHECK(frw && y && off, "taco_gl_frame_packed: NULL");
+    TACO_CHECK(B >= 1 && B <= 65535 && hop >= 1 && win_length >= 1 && win_length <= n_fft && max_frames >= 2 &&
+               hop * (max_frames - 1) > n_fft / 2, "taco_gl_frame_packed: bad sizes (max_frames=%d)", max_frames);
+    TACO_LAUNCH(gl_frame_kernel, packed_grid((int64_t)max_frames * n_fft, B), 256, 0, (cudaStream_t)stream, frw, y, 0, 0, hop, n_fft,
+                win_length, off, (int64_t)0);
+    TACO_LAUNCH_CHECK();
+    return 0;
+}
+
+int taco_speech_frames(int* frames, const float* spec, int B, int T, int r, int F, const float* scale, const float* shift,
+                       float top_db, void* stream) {
+    TACO_CHECK(frames && spec, "taco_speech_frames: NULL");
+    TACO_CHECK(B >= 1 && r >= 1 && T >= 4 && F >= 1, "taco_speech_frames: bad sizes (B=%d, T=%d, r=%d, F=%d)", B, T, r, F);
+    TACO_CHECK(top_db > 0.f && top_db <= FLT_MAX, "taco_speech_frames: top_db=%g must be finite and positive", (double)top_db);
+    TACO_CHECK((scale == nullptr) == (shift == nullptr), "taco_speech_frames: scale and shift go together");
+    const int n = 4 * r * (T / 4);
+    const int64_t total = (int64_t)B * n;
+    cudaStream_t st = (cudaStream_t)stream;
+    float* e = nullptr;                                                 // e[B][n], stream-ordered: no host synchronisation
+#ifdef TACO_HOST_EMU
+    e = static_cast<float*>(malloc((size_t)total * sizeof(float)));
+    TACO_CHECK(e, "taco_speech_frames: out of memory");
+#else
+    TACO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&e), (size_t)total * sizeof(float), st));
+#endif
+    int64_t g = (total + SF_THREADS / 32 - 1) / (SF_THREADS / 32);
+    if (g > TACO_SMS * 16) g = TACO_SMS * 16;
+    TACO_LAUNCH(frame_power_kernel, (int)g, SF_THREADS, 0, st, e, spec, T, n, r, F, scale, shift, total);
+    TACO_LAUNCH_CHECK();
+    TACO_LAUNCH(speech_end_kernel, B, SF_THREADS, 0, st, frames, e, n, r, T, top_db);
+    TACO_LAUNCH_CHECK();
+#ifdef TACO_HOST_EMU
+    free(e);
+#else
+    TACO_CUDA(cudaFreeAsync(e, st));
+#endif
     return 0;
 }
 

@@ -411,6 +411,68 @@ def irfft2048(x, X):
     L.check(L.lib().taco_irfft2048(_p(x), _p(X), x.numel() // 2048, _st()), "taco_irfft2048")
 
 
+def _affine(scale, shift, W, name):
+    if (scale is None) != (shift is None):
+        raise L.TacoError(f"{name}: scale and shift go together")
+    for t, nm in ((scale, "scale"), (shift, "shift")):
+        if t is not None:
+            _f32c(t, f"{name} {nm}")
+            if t.dtype != torch.float32 or t.numel() != W:
+                raise L.TacoError(f"{name}: {nm} must be fp32 [{W}], got {t.dtype} {tuple(t.shape)}")
+
+
+def speech_frames(frames, spec, r, scale=None, shift=None, top_db=60.0):
+    """frames int32 [B] = STFT frames to keep of each utterance of spec fp32 [B, T, F*r] (the post-net output): whole
+    blocks of 4r frames up to the last one within top_db of the utterance's loudest (tests/mirror_kernels_trim.py)"""
+    B, T, W = spec.shape
+    _f32c(spec, "speech_frames spec"); _cuda_c(frames, torch.int32, "speech_frames frames")
+    if spec.dtype != torch.float32 or W % r or frames.shape != (B,):
+        raise L.TacoError(f"speech_frames: spec fp32 [B, T, F*r] (r={r}) and frames [B], got {spec.dtype} "
+                          f"{tuple(spec.shape)} and {tuple(frames.shape)}")
+    _affine(scale, shift, W, "speech_frames")
+    L.check(L.lib().taco_speech_frames(_p(frames), _p(spec), B, T, r, W // r, _p(scale), _p(shift), float(top_db), _st()),
+            "taco_speech_frames")
+
+
+def _packed(off, name):
+    _cuda_c(off, torch.int64, f"{name} off")
+    if off.dim() != 1 or off.numel() < 2:
+        raise L.TacoError(f"{name}: off must be int64 [B+1], got {tuple(off.shape)}")
+    return off.numel() - 1
+
+
+def gl_init_packed(full, mag, spec, phase_u, off, r, max_frames, scale=None, shift=None):
+    """gl_init over the packed layout: utterance b owns rows off[b]:off[b+1] of mag / full / phase_u [N, F]"""
+    N, F = mag.shape
+    for t, nm in ((full, "full"), (mag, "mag"), (spec, "spec"), (phase_u, "phase_u")):
+        _f32c(t, f"gl_init_packed {nm}")
+    B = _packed(off, "gl_init_packed")
+    assert full.dtype == torch.complex64 and spec.dtype == mag.dtype == phase_u.dtype == torch.float32
+    assert full.shape == phase_u.shape == (N, F) and spec.dim() == 3 and spec.shape[0] == B and spec.shape[2] == F * r
+    _affine(scale, shift, F * r, "gl_init_packed")
+    L.check(L.lib().taco_gl_init_packed(_p(full), _p(mag), _p(spec), _p(phase_u), _p(off), B, spec.shape[1], r, F, int(max_frames),
+                                        _p(scale), _p(shift), _st()), "taco_gl_init_packed")
+
+
+def gl_ola_packed(y, fr, off, max_frames, hop, win_length):
+    """gl_ola over the packed layout: fr [N, n_fft] -> y [hop*(N - B)], utterance b's samples from hop*(off[b] - b)"""
+    N, n_fft = fr.shape
+    _f32c(y, "gl_ola_packed y"); _f32c(fr, "gl_ola_packed fr")
+    B = _packed(off, "gl_ola_packed")
+    assert y.dtype == fr.dtype == torch.float32 and y.shape == (hop * (N - B),)
+    L.check(L.lib().taco_gl_ola_packed(_p(y), _p(fr), _p(off), B, int(max_frames), hop, n_fft, win_length, _st()), "taco_gl_ola_packed")
+
+
+def gl_frame_packed(frw, y, off, max_frames, hop, win_length):
+    """gl_frame over the packed layout: y [hop*(N - B)] -> frw [N, n_fft]"""
+    N, n_fft = frw.shape
+    _f32c(y, "gl_frame_packed y"); _f32c(frw, "gl_frame_packed frw")
+    B = _packed(off, "gl_frame_packed")
+    assert y.dtype == frw.dtype == torch.float32 and y.shape == (hop * (N - B),)
+    L.check(L.lib().taco_gl_frame_packed(_p(frw), _p(y), _p(off), B, int(max_frames), hop, n_fft, win_length, _st()),
+            "taco_gl_frame_packed")
+
+
 def normalize_f16(out, x, mean, std):
     """out fp32 [..., W] = the reference's in-place float16 normalisation of x (float16) followed by the float32 cast"""
     W = x.shape[-1]

@@ -9,6 +9,15 @@ output is de-normalised with the checkpoint's ``stft_mean`` / ``stft_std`` and i
 (test.py:59-64).  The waveform is written as ``log/<save_path>/test/<n>.wav`` and the alignment as
 ``<n>_attention.npy``; with ``--summaries`` the reference's TensorBoard audio and image summaries go next to them
 (:33, :65-69; tacotron_b200/summary.py).
+
+    echo "a prompt to say" | python -m tacotron_b200.test -t nancy --trim-tail
+
+``--trim-tail`` ends each utterance where its speech ends instead of after ``max_decode_iter * r`` frames: the end is
+found on the device (``audio.speech_frames``: the last STFT frame within 60 dB of the utterance's loudest, rounded up to
+whole decoder-step blocks) and Griffin-Lim inverts only the frames up to it (``audio.invert_speech``).  The WAV, the
+attention array (the first ``frames/r`` decoder steps) and the summaries then end there too.  The rule rests on the
+training targets, which end in ``log(1e-8)`` padding frames; it has not been observed on a trained model's output.
+Without the flag every file is what the driver writes without it.
 """
 from __future__ import annotations
 
@@ -20,9 +29,9 @@ import numpy as np
 import torch
 
 
-def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None):
+def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, trim_tail=False):
     """summary_dir: also write each prompt's audio and attention image as TensorBoard summaries there, at step 0
-    (tacotron_b200/summary.py)"""
+    (tacotron_b200/summary.py).  trim_tail: end each utterance where its speech ends (module docstring)."""
     from . import audio, checkpoint, data_input
     from .train import write_wav
     sr = 24000 if "blizzard" in config.data_path else 16000                              # test.py:15
@@ -73,10 +82,17 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None):
             _, outputs = model.inference(inputs, train=False)
             alignments = model.alignments
             log("saving samples")
-            wav = audio.invert_spectrogram(outputs, config.r, stft_mean=mean_d, stft_std=std_d)   # :64, batched on the device
+            if trim_tail:
+                frames = audio.speech_frames(outputs, config.r, stft_mean=mean_d, stft_std=std_d)
+                wav = audio.invert_speech(outputs, config.r, frames, stft_mean=mean_d, stft_std=std_d)
+                steps = (frames.cpu() // config.r).tolist()
+            else:
+                wav = audio.invert_spectrogram(outputs, config.r, stft_mean=mean_d, stft_std=std_d)   # :64, batched on the device
             for b in range(outputs.shape[0]):                                            # :59-70
                 text = "".join(ivocab[int(w)] for w in inputs["text"][b].cpu().numpy())
                 wave, alignment = wav[b].cpu().numpy(), alignments[b].cpu().numpy()
+                if trim_tail:
+                    alignment = alignment[:steps[b]]
                 write_wav(os.path.join(out_dir, f"{n}.wav"), wave, sr)
                 np.save(os.path.join(out_dir, f"{n}_attention.npy"), alignment)
                 with open(os.path.join(out_dir, f"{n}.txt"), "w") as f:
@@ -98,6 +114,8 @@ def main(argv=None):
     parser.add_argument("-t", "--train-set", default="nancy")
     parser.add_argument("-s", "--speaker", type=int, default=0, help="speaker id of a multi-speaker model")
     parser.add_argument("--summaries", action="store_true", help="write TensorBoard summaries to log/<save_path>/test")
+    parser.add_argument("--trim-tail", action="store_true",
+                        help="end each utterance where its speech ends and invert only those frames")
     parser.add_argument("--max-ctas", type=int, default=None,
                         help="CTAs (SMs) the decoder kernels may occupy, at least 32 (default: all the device holds)")
     args = parser.parse_args(argv)
@@ -109,7 +127,7 @@ def main(argv=None):
     config.max_ctas = args.max_ctas
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "test") if args.summaries else None      # test.py:33
-    test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir)
+    test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir, trim_tail=args.trim_tail)
 
 
 if __name__ == "__main__":
