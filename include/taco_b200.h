@@ -381,6 +381,27 @@ int taco_gl_ola_packed(float* y, const float* fr, const int64_t* off, int B, int
                        int win_length, void* stream);
 int taco_gl_frame_packed(float* frw, const float* y, const int64_t* off, int B, int max_frames, int hop, int n_fft,
                          int win_length, void* stream);
+/* Where each utterance's speech starts and ends, for long-form synthesis (tacotron_b200.audio.speech_bounds): the frame
+ * space, log power and voiced rule of taco_speech_frames, and writes bounds[b] = {f0, f1, frames}:
+ *   - f0 = the first voiced frame, f1 = the last voiced frame + 1;
+ *   - frames = exactly the value taco_speech_frames writes for frames[b] (Griffin-Lim's frame count);
+ *   - {0, n, n} when any e[f] or E is not finite.
+ * Two launches (taco_speech_frames' per-frame power kernel, then one CTA per utterance) and a stream-ordered scratch of
+ * B*n floats; no host synchronisation.  Same argument rules as taco_speech_frames.
+ * Semantics: tests/longform_oracle.py speech_bounds.                                                                     */
+int taco_speech_bounds(int* bounds, const float* spec, int B, int T, int r, int F, const float* scale, const float* shift,
+                       float top_db, void* stream);
+/* Join synthesised pieces into one waveform (tacotron_b200.audio.join_speech): seg int64 [S][3], segment s =
+ * {src_start, dst_start, len}, sets out[dst_start + i] = src[src_start + i] * w(i), i in [0, len), with
+ *   - w(i) = min(1, c(i), c(len-1-i)), c(j) = 0.5 - 0.5 cos(pi (j + 0.5) / fade) for j < fade and 1 otherwise: a
+ *     raised-cosine fade-in and fade-out of `fade` samples at every cut (evaluated as sin^2 in double, so the product is
+ *     one rounding from the exact value);
+ *   - samples of out that no segment covers are not written (the caller zero-fills out, so gaps are silence).
+ * One launch (blockIdx.y = segment, x over samples); max_len (the largest len) sizes the grid.  The caller checks that
+ * every segment lies inside src and out and that no two overlap in out; a segment outside [0, out_len) is skipped.
+ * 1 <= S <= 65535, out_len >= 0, max_len >= 0, fade >= 1.  Semantics: tests/longform_oracle.py join_segments.          */
+int taco_join_segments(float* out, int64_t out_len, const float* src, const int64_t* seg, int S, int max_len, int fade,
+                       void* stream);
 
 /* Input data format (SURVEY 8(f) rank 3): spectrograms are stored float16 (preprocess.py:179-180) and normalised in
  * that dtype (data_input.py:56-64) before the float32 cast (:38-39).  Bit-exact device version of those statements:

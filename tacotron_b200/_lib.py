@@ -110,6 +110,8 @@ EXPORTS = [
     "taco_gl_init", "taco_gl_ola", "taco_gl_frame", "taco_gl_phase", "taco_rfft2048", "taco_irfft2048",
     # end of speech and the packed Griffin-Lim kernels (synthesis tail trim)
     "taco_speech_frames", "taco_gl_init_packed", "taco_gl_ola_packed", "taco_gl_frame_packed",
+    # where speech starts and ends, and the join of synthesised pieces (long-form synthesis)
+    "taco_speech_bounds", "taco_join_segments",
     # input data format
     "taco_normalize_f16",
     # feature extraction (preprocessing)
@@ -186,6 +188,8 @@ def lib():
     L.taco_gl_init_packed.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     L.taco_gl_ola_packed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
     L.taco_gl_frame_packed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    L.taco_speech_bounds.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]
+    L.taco_join_segments.argtypes = [vp, i64, vp, vp, i32, i32, i32, vp]
     L.taco_normalize_f16.argtypes = [vp, vp, vp, vp, i64, i32, vp]
     L.taco_trim_bounds.argtypes = [vp, vp, vp, i32, i32, i32, f32, vp]
     L.taco_feature_frames.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]

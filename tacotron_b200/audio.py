@@ -380,6 +380,13 @@ def invert_speech(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, pha
     frames are packed end to end, so one iteration is still 5 launches; utterance b equals invert_spectrogram on
     spec[b:b+1, :frames[b]//r] with the same initial phases.  phase_u: packed uniform [0,1) phases [sum(frames), 1025],
     drawn on the device if None.  Reads frames to the host once."""
+    y, start = invert_speech_packed(spec, r, frames, n_iter, stft_mean, stft_std, phase_u, K, generator)
+    return [y[start[b]:start[b + 1]] for b in range(len(start) - 1)]
+
+
+def invert_speech_packed(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, generator=None):
+    """invert_speech's waveforms as the one flat buffer Griffin-Lim writes: (y, start) with utterance b in
+    y[start[b]:start[b+1]] (start int64 numpy [B+1])"""
     K = K or _K()
     B, T, W = spec.shape
     assert W == F_BINS * r, (W, r)
@@ -407,7 +414,36 @@ def invert_speech(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, pha
     frw = torch.empty((N, n_fft), dtype=rdt, device=dev)
     _gl_iterations(K, full, mag, spec.contiguous(), phase_u.contiguous(), r, scale, shift, y, frw, n_iter,
                    packed=(torch.from_numpy(off).to(dev), nmax))
-    return [y[hop_length * (off[b] - b):hop_length * (off[b + 1] - b - 1)] for b in range(B)]
+    return y, hop_length * (off - np.arange(B + 1))
+
+
+def speech_bounds(spec, r, stft_mean=None, stft_std=None, top_db=TRIM_TOP_DB, K=None):
+    """Where each utterance's speech starts and ends in spec [B, T, 1025*r] (de-normalised like speech_frames) -> int32
+    [B, 3] on spec's device, without a host synchronisation: {f0, f1, frames} = the first voiced STFT frame, the last
+    voiced frame + 1, and exactly speech_frames' frame count; {0, n, n} when the spectrogram is not finite."""
+    K = K or _K()
+    scale, shift = (stft_std, stft_mean) if stft_std is not None else (None, None)
+    bounds = torch.empty((spec.shape[0], 3), dtype=torch.int32, device=spec.device)
+    K.speech_bounds(bounds, spec.contiguous(), r, scale, shift, top_db)
+    return bounds
+
+
+JOIN_FADE_S = 0.01      # raised-cosine fade at every cut of a joined waveform
+
+
+def kept_samples(f0, f1, frames):
+    """samples [a, b) of an utterance's invert_speech output (hop*(frames-1) samples) that long-form synthesis keeps for
+    speech bounds (f0, f1): from one hop before the first voiced frame to the last voiced frame's hop"""
+    L = hop_length * (frames - 1)
+    return max(hop_length * (f0 - 1), 0), min(hop_length * f1, L)
+
+
+def join_speech(out, src, seg, sr, K=None):
+    """out[d:d+n] = src[a:a+n] with a raised-cosine fade of 10 ms (JOIN_FADE_S at sr) at both ends, for every row
+    {a, d, n} of seg int64 [S, 3] (host); one launch.  The segments must lie inside src and out and not overlap in out;
+    samples of out outside them are left as they are."""
+    K = K or _K()
+    K.join_segments(out, src, seg, max(1, int(round(sr * JOIN_FADE_S))))
 
 
 class GriffinLimGraph:

@@ -228,6 +228,90 @@ __global__ void __launch_bounds__(SF_THREADS) speech_end_kernel(int* __restrict_
     }
 }
 
+// one CTA per utterance, speech_end_kernel's rule plus the first voiced frame: bounds[b] = {f0, f1, frames} with
+// f0 = the first f with e[f] >= thr, f1 = the last such f + 1, frames = speech_end_kernel's frames[b]; {0, n, n} if any
+// e[f] is not finite.  The max is order-independent and thr is the same expression, so frames is bit for bit the same.
+__global__ void __launch_bounds__(SF_THREADS) speech_bounds_kernel(int* __restrict__ bounds, const float* __restrict__ e, int n,
+                                                                   int r, int T, float top_db) {
+    __shared__ float rmax[SF_THREADS];
+    __shared__ int rfirst[SF_THREADS], rlast[SF_THREADS];
+    const int tid = threadIdx.x;
+    const float* eb = e + (int64_t)blockIdx.x * n;
+    float m = -INFINITY;
+    int bad = 0;
+    for (int f = tid; f < n; f += SF_THREADS) {
+        const float x = eb[f];
+        if (fabsf(x) <= FLT_MAX) m = fmaxf(m, x);
+        else bad = 1;
+    }
+    rmax[tid] = m;
+    rlast[tid] = bad;
+    __syncthreads();
+    for (int s = SF_THREADS / 2; s > 0; s >>= 1) {
+        if (tid < s) {
+            rmax[tid] = fmaxf(rmax[tid], rmax[tid + s]);
+            rlast[tid] |= rlast[tid + s];
+        }
+        __syncthreads();
+    }
+    const float thr = rmax[0] - top_db * 0.230258509299404568f;       // ln(10) / 10, as in speech_end_kernel
+    bad = rlast[0];
+    __syncthreads();
+    int first = n, last = -1;
+    for (int f = tid; f < n; f += SF_THREADS)
+        if (eb[f] >= thr) {
+            first = min(first, f);
+            last = f;
+        }
+    rfirst[tid] = first;
+    rlast[tid] = last;
+    __syncthreads();
+    for (int s = SF_THREADS / 2; s > 0; s >>= 1) {
+        if (tid < s) {
+            rfirst[tid] = min(rfirst[tid], rfirst[tid + s]);
+            rlast[tid] = max(rlast[tid], rlast[tid + s]);
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        const int blk = 4 * r;
+        int k = (rlast[0] + blk) / blk;
+        const int kmin = (5 + blk - 1) / blk;
+        if (k < kmin) k = kmin;
+        if (k > T / 4) k = T / 4;
+        int* o = bounds + 3 * (int64_t)blockIdx.x;
+        o[0] = bad ? 0 : rfirst[0];
+        o[1] = bad ? n : rlast[0] + 1;
+        o[2] = bad ? n : blk * k;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Joining synthesised pieces (taco_join_segments): blockIdx.y = segment s = {src_start, dst_start, len}, a grid-stride
+// loop over its samples; out[dst_start + i] = src[src_start + i] * w(i), w(i) = min(1, c(i), c(len-1-i)),
+// c(j) = 0.5 - 0.5 cos(pi (j + 0.5) / fade) for j < fade, 1 otherwise.  c is evaluated as sin^2(pi (j + 0.5) / (2 fade))
+// in double: the same raised cosine without the cancellation of 1 - cos near j = 0, so the product is rounded once from
+// a weight exact to ~1e-15.  A segment outside [0, out_len) is skipped (the host has validated them all).
+// ---------------------------------------------------------------------------------------------------------------------
+#ifdef TACO_HOST_EMU
+inline double sinpi(double x) { return std::sin(M_PI * x); }
+#endif
+__device__ __forceinline__ double fade_weight(int64_t j, int fade) {
+    if (j >= fade) return 1.0;
+    const double s = sinpi(0.5 * ((double)j + 0.5) / (double)fade);     // sinpi: no argument reduction, no stack frame
+    return s * s;
+}
+
+__global__ void join_segments_kernel(float* __restrict__ out, int64_t out_len, const float* __restrict__ src,
+                                     const int64_t* __restrict__ seg, int fade) {
+    const int64_t s0 = seg[3 * (int64_t)blockIdx.y], d0 = seg[3 * (int64_t)blockIdx.y + 1], len = seg[3 * (int64_t)blockIdx.y + 2];
+    if (s0 < 0 || d0 < 0 || len < 0 || d0 > out_len - len) return;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < len; i += (int64_t)gridDim.x * blockDim.x) {
+        const double w = fmin(1.0, fmin(fade_weight(i, fade), fade_weight(len - 1 - i, fade)));
+        out[d0 + i] = (float)((double)src[s0 + i] * w);
+    }
+}
+
 
 // ---------------------------------------------------------------------------------------------------------------------
 // 2048-point REAL FFT pair in shared memory.  The real row is transformed as a 1024-point COMPLEX sequence
@@ -425,6 +509,47 @@ int taco_speech_frames(int* frames, const float* spec, int B, int T, int r, int 
 #else
     TACO_CUDA(cudaFreeAsync(e, st));
 #endif
+    return 0;
+}
+
+int taco_speech_bounds(int* bounds, const float* spec, int B, int T, int r, int F, const float* scale, const float* shift,
+                       float top_db, void* stream) {
+    TACO_CHECK(bounds && spec, "taco_speech_bounds: NULL");
+    TACO_CHECK(B >= 1 && r >= 1 && T >= 4 && F >= 1, "taco_speech_bounds: bad sizes (B=%d, T=%d, r=%d, F=%d)", B, T, r, F);
+    TACO_CHECK(top_db > 0.f && top_db <= FLT_MAX, "taco_speech_bounds: top_db=%g must be finite and positive", (double)top_db);
+    TACO_CHECK((scale == nullptr) == (shift == nullptr), "taco_speech_bounds: scale and shift go together");
+    const int n = 4 * r * (T / 4);
+    const int64_t total = (int64_t)B * n;
+    cudaStream_t st = (cudaStream_t)stream;
+    float* e = nullptr;                                                 // e[B][n], stream-ordered, as in taco_speech_frames
+#ifdef TACO_HOST_EMU
+    e = static_cast<float*>(malloc((size_t)total * sizeof(float)));
+    TACO_CHECK(e, "taco_speech_bounds: out of memory");
+#else
+    TACO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&e), (size_t)total * sizeof(float), st));
+#endif
+    int64_t g = (total + SF_THREADS / 32 - 1) / (SF_THREADS / 32);
+    if (g > TACO_SMS * 16) g = TACO_SMS * 16;
+    TACO_LAUNCH(frame_power_kernel, (int)g, SF_THREADS, 0, st, e, spec, T, n, r, F, scale, shift, total);
+    TACO_LAUNCH_CHECK();
+    TACO_LAUNCH(speech_bounds_kernel, B, SF_THREADS, 0, st, bounds, e, n, r, T, top_db);
+    TACO_LAUNCH_CHECK();
+#ifdef TACO_HOST_EMU
+    free(e);
+#else
+    TACO_CUDA(cudaFreeAsync(e, st));
+#endif
+    return 0;
+}
+
+int taco_join_segments(float* out, int64_t out_len, const float* src, const int64_t* seg, int S, int max_len, int fade,
+                       void* stream) {
+    TACO_CHECK(out && src && seg, "taco_join_segments: NULL");
+    TACO_CHECK(S >= 1 && S <= 65535 && out_len >= 0 && max_len >= 0 && fade >= 1,
+               "taco_join_segments: bad sizes (S=%d, out_len=%lld, max_len=%d, fade=%d)", S, (long long)out_len, max_len, fade);
+    if (max_len == 0) return 0;
+    TACO_LAUNCH(join_segments_kernel, packed_grid(max_len, S), 256, 0, (cudaStream_t)stream, out, out_len, src, seg, fade);
+    TACO_LAUNCH_CHECK();
     return 0;
 }
 

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -432,6 +433,54 @@ def speech_frames(frames, spec, r, scale=None, shift=None, top_db=60.0):
     _affine(scale, shift, W, "speech_frames")
     L.check(L.lib().taco_speech_frames(_p(frames), _p(spec), B, T, r, W // r, _p(scale), _p(shift), float(top_db), _st()),
             "taco_speech_frames")
+
+
+def speech_bounds(bounds, spec, r, scale=None, shift=None, top_db=60.0):
+    """bounds int32 [B, 3] = {first voiced frame, last voiced frame + 1, speech_frames' frame count} of each utterance of
+    spec fp32 [B, T, F*r] (tests/longform_oracle.py speech_bounds)"""
+    B, T, W = spec.shape
+    _f32c(spec, "speech_bounds spec"); _cuda_c(bounds, torch.int32, "speech_bounds bounds")
+    if spec.dtype != torch.float32 or W % r or bounds.shape != (B, 3):
+        raise L.TacoError(f"speech_bounds: spec fp32 [B, T, F*r] (r={r}) and bounds [B, 3], got {spec.dtype} "
+                          f"{tuple(spec.shape)} and {tuple(bounds.shape)}")
+    _affine(scale, shift, W, "speech_bounds")
+    L.check(L.lib().taco_speech_bounds(_p(bounds), _p(spec), B, T, r, W // r, _p(scale), _p(shift), float(top_db), _st()),
+            "taco_speech_bounds")
+
+
+def check_segments(seg, src_len, out_len):
+    """seg int64 [S, 3] rows {src_start, dst_start, len}: every segment inside src [0, src_len) and out [0, out_len),
+    no two overlapping in out; raises ValueError naming the first that is not"""
+    seg = np.asarray(seg, dtype=np.int64).reshape(-1, 3)
+    for s, (a, d, n) in enumerate(seg.tolist()):
+        if n < 0 or a < 0 or d < 0 or a + n > src_len or d + n > out_len:
+            raise ValueError(f"join_segments: segment {s} = (src {a}, dst {d}, len {n}) outside src [0, {src_len}) or "
+                             f"out [0, {out_len})")
+    order = np.argsort(seg[:, 1], kind="stable")
+    ends = seg[order, 1] + seg[order, 2]
+    clash = np.flatnonzero(seg[order[1:], 1] < ends[:-1])
+    if clash.size:
+        i, j = int(order[clash[0]]), int(order[clash[0] + 1])
+        raise ValueError(f"join_segments: segments {i} and {j} overlap in out")
+    return seg
+
+
+def join_segments(out, src, seg, fade):
+    """out fp32 [out_len]: out[d + i] = src[a + i] * w(i) for every host row {a, d, len} of seg int64 [S, 3], w the
+    raised-cosine fade of `fade` samples at both ends (tests/longform_oracle.py join_segments); other samples of out are
+    left as they are.  The segments are checked on the host, then copied to the device: one launch."""
+    _f32c(out, "join_segments out"); _f32c(src, "join_segments src")
+    if out.dtype != torch.float32 or src.dtype != torch.float32 or out.dim() != 1 or src.dim() != 1:
+        raise L.TacoError(f"join_segments: out and src must be 1-D fp32, got {out.dtype} {tuple(out.shape)} and "
+                          f"{src.dtype} {tuple(src.shape)}")
+    seg = check_segments(seg, src.numel(), out.numel())
+    if len(seg) == 0:
+        return
+    if len(seg) > 65535 or int(seg[:, 2].max()) > 2**31 - 1:
+        raise ValueError(f"join_segments: at most 65535 segments of < 2^31 samples per launch, got {len(seg)}")
+    seg_d = torch.from_numpy(np.ascontiguousarray(seg)).to(out.device)
+    L.check(L.lib().taco_join_segments(_p(out), out.numel(), _p(src), _p(seg_d), len(seg), int(seg[:, 2].max()), int(fade),
+                                       _st()), "taco_join_segments")
 
 
 def _packed(off, name):

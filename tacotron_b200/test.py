@@ -18,6 +18,22 @@ whole decoder-step blocks) and Griffin-Lim inverts only the frames up to it (``a
 attention array (the first ``frames/r`` decoder steps) and the summaries then end there too.  The rule rests on the
 training targets, which end in ``log(1e-8)`` padding frames; it has not been observed on a trained model's output.
 Without the flag every file is what the driver writes without it.
+
+    python -m tacotron_b200.test -t nancy --long-form < paragraph.txt
+
+``--long-form`` speaks each stdin line as one clip, whatever its length (without it, a line over 140 vocabulary
+characters is an error and a line that takes longer than ``max_decode_iter * r`` frames to say is cut off).  Each line is
+split into chunks at sentence ends, clause breaks or spaces (``tacotron_b200/longform.py``); the chunks of all lines are
+decoded in batches of at most 32, and ``audio.speech_bounds`` finds where each chunk's speech starts and ends on the
+device.  A chunk whose speech reaches its last frame most likely ran out of decoder steps: it is split again at the
+break nearest its middle and both halves go to the next round (a chunk with no break left is kept, with one logged
+warning).  That rule rests on the training targets, which end in ``log(1e-8)`` padding; it has not been observed on a
+trained model.  Each chunk's Griffin-Lim output is cut to its speech (``audio.kept_samples``) and the pieces of a line
+are joined with a pause set by the break between them and a 10 ms raised-cosine fade at every cut
+(``audio.join_speech``, one launch per batch into one zero-filled device buffer that holds every line).  Per line the
+driver writes ``<n>.wav``, ``<n>.txt`` (the whole line), ``<n>_chunks.txt`` (one chunk per line) and
+``<n>_attention.npy`` (the block-diagonal stack of the chunk alignments), and with ``--summaries`` one audio and one
+image summary.  ``--trim-tail`` changes nothing here: long-form already trims.
 """
 from __future__ import annotations
 
@@ -29,9 +45,10 @@ import numpy as np
 import torch
 
 
-def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, trim_tail=False):
+def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, trim_tail=False, long_form=False):
     """summary_dir: also write each prompt's audio and attention image as TensorBoard summaries there, at step 0
-    (tacotron_b200/summary.py).  trim_tail: end each utterance where its speech ends (module docstring)."""
+    (tacotron_b200/summary.py).  trim_tail: end each utterance where its speech ends; long_form: speak each line as one
+    clip, whatever its length (module docstring).  Returns one device waveform per prompt."""
     from . import audio, checkpoint, data_input
     from .train import write_wav
     sr = 24000 if "blizzard" in config.data_path else 16000                              # test.py:15
@@ -73,6 +90,13 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, tri
     if summary_dir is not None:                                                          # :33
         from . import summary
         writer, scopes = summary.EventWriter(summary_dir), summary.NameScopes()
+    if long_form:
+        try:
+            return _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, sr, log, writer,
+                              scopes if writer is not None else None)
+        finally:
+            if writer is not None:
+                writer.close()
     n = 0
     waves = []
     try:
@@ -109,6 +133,80 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, tri
     return waves
 
 
+def _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, sr, log, writer, scopes):
+    """test(long_form=True): the rounds of synthesis and re-splitting, then the join (module docstring)"""
+    from . import audio, data_input, longform
+    from .train import write_wav
+    r = config.r
+    vocab = set(ivocab.values())
+    lines = [longform.split_line(p, vocab, i) for i, p in enumerate(prompts)]
+    outs = []                # flat Griffin-Lim output of every synthesised batch
+    done = {}                # id(chunk) -> (batch, first sample of the chunk in it, (f0, f1, frames), alignment)
+    pending = [c for cs in lines for c in cs]
+    while pending:
+        again = []
+        for i in range(0, len(pending), data_input.BATCH_SIZE):
+            group = pending[i:i + data_input.BATCH_SIZE]
+            inputs = next(data_input.load_prompts([c.prompt for c in group], ivocab))
+            if config.num_speakers > 1:
+                inputs["speaker"] = torch.full((len(group),), speaker, dtype=torch.int32, device=inputs["text"].device)
+            _, outputs = model.inference(inputs, train=False)
+            bounds = audio.speech_bounds(outputs, r, stft_mean=mean_d, stft_std=std_d).cpu().numpy()    # the one read
+            y, start = audio.invert_speech_packed(outputs, r, bounds[:, 2], stft_mean=mean_d, stft_std=std_d)
+            align = model.alignments.cpu().numpy()
+            n = 4 * r * (outputs.shape[1] // 4)
+            outs.append(y)
+            for b, c in enumerate(group):
+                f0, f1, frames = (int(v) for v in bounds[b])
+                if f1 == n:                  # speech up to the last frame: most likely out of decoder steps
+                    halves = longform.resplit(c)
+                    if halves is not None:
+                        cs = lines[c.line]
+                        k = next(j for j, x in enumerate(cs) if x is c)
+                        cs[k:k + 1] = halves
+                        again.extend(halves)
+                        continue
+                    log(f"warning: line {c.line}: chunk {c.text!r} is voiced up to its last decoder step and has no break "
+                        f"left to split it at; kept as it is")
+                cols = min(len(c.prompt), data_input.MAX_TEXT_LEN)
+                done[id(c)] = (len(outs) - 1, int(start[b]), (f0, f1, frames), align[b, :frames // r, :cols])
+        pending = again
+    log("saving samples")
+    segs = {}                # batch -> rows {src_start, dst_start, len} of its join
+    spans = []
+    total = 0
+    for cs in lines:
+        kept = [audio.kept_samples(*done[id(c)][2]) for c in cs]
+        dst, length = longform.layout([e - a for a, e in kept], [c.brk for c in cs], sr)
+        for c, (a, e), d in zip(cs, kept, dst):
+            bi, s0 = done[id(c)][:2]
+            segs.setdefault(bi, []).append((s0 + a, total + d, e - a))
+        spans.append((total, length))
+        total += length
+    out = torch.zeros(total, dtype=torch.float32, device=mean_d.device)
+    for bi, rows in segs.items():
+        audio.join_speech(out, outs[bi], np.asarray(rows, dtype=np.int64), sr)
+    waves = []
+    for n, (cs, (o, length)) in enumerate(zip(lines, spans)):
+        wave = out[o:o + length]
+        w = wave.cpu().numpy()
+        alignment = longform.block_diagonal([done[id(c)][3] for c in cs])
+        text = prompts[n].rstrip("\r\n")
+        write_wav(os.path.join(out_dir, f"{n}.wav"), w, sr)
+        np.save(os.path.join(out_dir, f"{n}_attention.npy"), alignment)
+        with open(os.path.join(out_dir, f"{n}.txt"), "w") as f:
+            f.write(text)
+        with open(os.path.join(out_dir, f"{n}_chunks.txt"), "w") as f:
+            f.write("".join(c.text + "\n" for c in cs))
+        if writer is not None:
+            from . import summary
+            tag = summary.clean_tag(text)
+            writer.add(0, [summary.audio_value(scopes.unique(tag) + "/audio/0", w, sr),
+                           summary.image_value(scopes.unique(tag) + "/image/0", summary.attention_rgba(alignment))])
+        waves.append(wave)
+    return waves
+
+
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", "--train-set", default="nancy")
@@ -116,6 +214,9 @@ def main(argv=None):
     parser.add_argument("--summaries", action="store_true", help="write TensorBoard summaries to log/<save_path>/test")
     parser.add_argument("--trim-tail", action="store_true",
                         help="end each utterance where its speech ends and invert only those frames")
+    parser.add_argument("--long-form", action="store_true",
+                        help="speak each line as one clip, whatever its length: split at sentence and clause breaks, "
+                             "decode the pieces as batches and join them")
     parser.add_argument("--max-ctas", type=int, default=None,
                         help="CTAs (SMs) the decoder kernels may occupy, at least 32 (default: all the device holds)")
     args = parser.parse_args(argv)
@@ -127,7 +228,8 @@ def main(argv=None):
     config.max_ctas = args.max_ctas
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "test") if args.summaries else None      # test.py:33
-    test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir, trim_tail=args.trim_tail)
+    test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir, trim_tail=args.trim_tail,
+         long_form=args.long_form)
 
 
 if __name__ == "__main__":
