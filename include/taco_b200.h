@@ -318,12 +318,28 @@ typedef struct taco_decoder_bwd_args {
                                              min(budget, capacity, 128) CTAs                                */
     const float *H0[3];                   /* [B][256] initial state of GRU i (h_i(-1)), or NULL = zero        */
     float *DH0;                           /* out: [3][B][256] d(loss)/d(h_i(-1)), or NULL = not wanted        */
+    const float *dscore_add;              /* [B][T][Tx] added to the softmax backward's dscore of every step
+                                             before it feeds dpq and DSCORE (taco_guided_attention's
+                                             gradient), or NULL = nothing added, today's arithmetic        */
 } taco_decoder_bwd_args;
 size_t taco_decoder_bwd_workspace_bytes(void);
 int    taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream);
 /* dkeys[b][j][d] = sum_t DSCORE[b][t][j] v[d] (1-e^2); dv[d] += sum DSCORE e; e = tanh(keys + PQ[t][b]) */
 int taco_attn_bwd_post(float* dkeys, float* dv, const float* DSCORE, const float* keys, const float* PQ, const float* v,
                        int B, int T, int Tx, void* stream);
+/* (new; the reference has no such term) guided attention loss of Tachibana et al. 2017, "Efficiently Trainable
+ * Text-to-Speech System Based on Deep Convolutional Networks with Guided Attention", arXiv:1710.08969, on the alignments
+ * align [B][T][Tx] the forward saves.  With N_b = min(text_length[b], Tx) and T_b = speech_steps[b] (in [1, T]):
+ *     W[b][t][j] = 1 - exp(-(j/N_b - t/T_b)^2 / (2 g^2))  for t < T_b and j < N_b, else 0
+ *     loss[0]    = lam * sum_{b,t,j} align W                                   (a sum, like the two L1 losses)
+ *     dscore[b][t][j] = lam * align[b][t][j] * (W[b][t][j] - s[b][t]),  s = sum_j align W   (0 outside the mask)
+ * dscore is d(loss)/d(attention score): the input taco_decoder_bwd_args.dscore_add takes.  One warp per (b, t) row
+ * forms W, s and dscore together; the loss is reduced from per-row partials in a fixed order (double accumulation), so
+ * it is bit-identical run to run.  g > 0, lam >= 0, Tx <= 256; no host synchronisation.                          */
+int taco_guided_attention(float* dscore, float* loss, const float* align, const int32_t* text_length,
+                          const int32_t* speech_steps, int B, int T, int Tx, float g, float lam, float* partial_ws,
+                          void* stream);
+int taco_guided_attention_partial_count(int B, int T);   /* floats partial_ws must hold (one per row: B*T) */
 
 /* tf.clip_by_global_norm(cap_grads) + tf.train.AdamOptimizer (tacotron.py:170-184; SURVEY A.12) on the flat
  * parameter / gradient buffers: out = sum x^2 (deterministic); g *= clip/max(sqrt(sumsq), clip);

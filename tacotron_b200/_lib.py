@@ -83,7 +83,7 @@ class DecoderBwdArgs(C.Structure):
         ("DATT", C.c_void_p), ("DY", C.c_void_p), ("DPQ", C.c_void_p), ("DSCORE", C.c_void_p),
         ("DCTX", C.c_void_p), ("DG", C.c_void_p * 3), ("DC", C.c_void_p * 3), ("DZ", C.c_void_p), ("DPN2", C.c_void_p),
         ("DPN1", C.c_void_p), ("DX", C.c_void_p), ("workspace", C.c_void_p), ("max_ctas", C.c_int32),
-        ("H0", C.c_void_p * 3), ("DH0", C.c_void_p),
+        ("H0", C.c_void_p * 3), ("DH0", C.c_void_p), ("dscore_add", C.c_void_p),
     ]
 
 
@@ -106,6 +106,8 @@ EXPORTS = [
     "taco_maxpool_bwd", "taco_highway_fwd", "taco_highway_bwd", "taco_l1_bwd", "taco_l1_bwd_ld", "taco_scatter_add_rows", "taco_bigru_bwd", "taco_bigru_bwd_h0",
     "taco_dec_inputs", "taco_decoder_bwd_workspace_bytes", "taco_decoder_bwd", "taco_attn_bwd_post", "taco_sumsq",
     "taco_adam_step",
+    # guided attention loss (opt-in training term)
+    "taco_guided_attention", "taco_guided_attention_partial_count",
     # spectrogram inversion (Griffin-Lim glue kernels)
     "taco_gl_init", "taco_gl_ola", "taco_gl_frame", "taco_gl_phase", "taco_rfft2048", "taco_irfft2048",
     # end of speech and the packed Griffin-Lim kernels (synthesis tail trim)
@@ -178,6 +180,9 @@ def lib():
     L.taco_attn_bwd_post.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]
     L.taco_sumsq.argtypes = [vp, i64, vp, vp, vp]
     L.taco_adam_step.argtypes = [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp, vp]
+    L.taco_guided_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, vp, vp]
+    L.taco_guided_attention_partial_count.argtypes = [i32, i32]
+    L.taco_guided_attention_partial_count.restype = C.c_int
     L.taco_gl_init.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
     L.taco_gl_ola.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]
     L.taco_gl_frame.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]

@@ -59,6 +59,7 @@ struct DecBwdP {
     float *DATT, *DY, *DPQ, *DSCORE, *DCTX, *DG[3], *DC[3], *DZ, *DPN2, *DPN1, *DX;
     const float *M124, *M7, *E;   // fused weights [U][768], [640][U]; E = dy_ext . W_out^T  [T][B][U]   (workspace, see host)
     const float* H0[3];           // [B][U] initial states h_i(-1), or NULL (zero state)
+    const float* dscore_add;      // [B][T][Tx] added to the softmax backward's dscore (guided attention), or NULL
     float* ws;
     unsigned int* bar;       // grid-barrier counter (zeroed by the host before the launch)
     int cache_weights;       // 1: this CTA's weight rows fit in shared memory (the normal case); 0: read them from L2
@@ -85,6 +86,7 @@ constexpr int WS_TOTAL = WS_E + WS_MAXT * RB * U;
 // 255 KB of code and every stage started with a cold instruction cache (ncu: 11 % issue utilisation, 13 K cycles per stage).
 #ifdef TACO_HOST_EMU
 #define TACO_NOINLINE
+static inline float __fadd_rn(float a, float b) { return a + b; }     // (host: one IEEE add, like the device intrinsic)
 #else
 #define TACO_NOINLINE __noinline__
 #endif
@@ -306,6 +308,8 @@ __global__ void __launch_bounds__(256, 1) decoder_bwd_kernel(const DecBwdP p) {
                 }
                 __syncthreads();
                 const float aj = (tid < Tx) ? __ldg(p.align + ((int64_t)b * T + t) * Tx + tid) : 0.f;
+                // issued with the align load, so its L2 latency overlaps the reduction below instead of following it
+                const float dsa = (p.dscore_add && tid < Tx) ? __ldg(p.dscore_add + ((int64_t)b * T + t) * Tx + tid) : 0.f;
                 float part = (tid < Tx) ? aj * dal_s[tid] : 0.f;
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
@@ -315,7 +319,8 @@ __global__ void __launch_bounds__(256, 1) decoder_bwd_kernel(const DecBwdP p) {
 #pragma unroll
                 for (int w = 0; w < NW; ++w) tot += red_s[w];
                 if (tid < Tx) {                                              // softmax backward
-                    const float ds = aj * (dal_s[tid] - tot);
+                    float ds = aj * (dal_s[tid] - tot);
+                    if (p.dscore_add) ds = __fadd_rn(ds, dsa);            // (never fused with the product: NULL keeps it as it was)
                     ds_s[tid] = ds;
                     p.DSCORE[((int64_t)b * T + t) * Tx + tid] = ds;
                 }
@@ -523,6 +528,7 @@ extern "C" int taco_decoder_bwd(const taco_decoder_bwd_args* a, void* stream) {
     p.dy_ext = a->dy_ext; p.align = a->align; p.values = a->values; p.keys = a->keys; p.PQ = a->PQ; p.PN1 = a->PN1; p.PN2 = a->PN2;
     p.sel = a->sel;
     for (int i = 0; i < 3; ++i) p.H0[i] = a->H0[i];
+    p.dscore_add = a->dscore_add;
     p.DATT = a->DATT; p.DY = a->DY; p.DPQ = a->DPQ; p.DSCORE = a->DSCORE; p.DCTX = a->DCTX; p.DZ = a->DZ; p.DPN2 = a->DPN2;
     p.DPN1 = a->DPN1; p.DX = a->DX;
     p.ws = a->workspace;

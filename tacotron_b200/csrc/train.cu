@@ -549,6 +549,66 @@ __global__ void __launch_bounds__(256) colsum_seg_kernel(float* __restrict__ out
     }
 }
 
+// guided attention (Tachibana et al. 2017): one warp per (b, t) row of the alignments.  The lane's up-to-8 positions
+// j = lane + 32 i are loaded at once; W, s = sum_j align W and the gradient lam align (W - s) are formed from the same
+// registers, so the loss and its gradient see the same W.  row_s[row] = s (the loss' per-row partial).
+constexpr int GA_WARPS = 8;
+constexpr int GA_PER_LANE = 256 / 32;        // Tx <= 256
+__global__ void __launch_bounds__(256) guided_attention_kernel(float* __restrict__ dscore, float* __restrict__ row_s,
+                                                               const float* __restrict__ align,
+                                                               const int32_t* __restrict__ text_length,
+                                                               const int32_t* __restrict__ speech_steps, int B, int T,
+                                                               int Tx, float inv_2g2, float lam) {
+    const int lane = threadIdx.x & 31;
+    const int64_t rows = (int64_t)B * T;
+    for (int64_t row = (int64_t)blockIdx.x * GA_WARPS + (threadIdx.x >> 5); row < rows; row += (int64_t)gridDim.x * GA_WARPS) {
+        const int b = (int)(row / T), t = (int)(row - (int64_t)b * T);
+        const int n = min(text_length[b], Tx);
+        const int tb = speech_steps[b];
+        const int nlive = (t < tb && n > 0) ? n : 0;     // positions j < nlive are inside the mask
+        const float* a = align + row * Tx;
+        float al[GA_PER_LANE], w[GA_PER_LANE];
+#pragma unroll
+        for (int i = 0; i < GA_PER_LANE; ++i) {
+            const int j = lane + 32 * i;
+            al[i] = (j < nlive) ? a[j] : 0.f;
+        }
+        float s = 0.f;
+#pragma unroll
+        for (int i = 0; i < GA_PER_LANE; ++i) {
+            const int j = lane + 32 * i;
+            w[i] = 0.f;
+            if (j < nlive) {
+                const float d = (float)j / (float)n - (float)t / (float)tb;
+                w[i] = -expm1f(-d * d * inv_2g2);        // 1 - exp(-x), accurate near the diagonal where W -> 0
+            }
+            s = fmaf(al[i], w[i], s);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+#pragma unroll
+        for (int i = 0; i < GA_PER_LANE; ++i) {
+            const int j = lane + 32 * i;
+            if (j < Tx) dscore[row * Tx + j] = (j < nlive) ? lam * al[i] * (w[i] - s) : 0.f;
+        }
+        if (lane == 0) row_s[row] = s;
+    }
+}
+// loss = lam * sum of the row partials: fixed per-thread strides, then thread 0 adds the 256 double sums in order
+__global__ void __launch_bounds__(256) guided_attention_sum_kernel(const float* __restrict__ row_s, int64_t rows, double lam,
+                                                                   float* __restrict__ loss) {
+    __shared__ double red[256];
+    double acc = 0.0;
+    for (int64_t i = threadIdx.x; i < rows; i += 256) acc += (double)row_s[i];
+    red[threadIdx.x] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double tot = 0.0;
+        for (int k = 0; k < 256; ++k) tot += red[k];
+        loss[0] = (float)(lam * tot);
+    }
+}
+
 }  // namespace
 
 static int g_gemm_impl = 0;        // taco_set_gemm_impl
@@ -603,6 +663,29 @@ int taco_colsum_seg(float* out, int64_t ldo, const float* A, int64_t lda, int M,
                "taco_colsum_seg: bad arguments (M=%d N=%d period=%d)", M, N, period);
     if (M == 0 || N == 0) return 0;
     TACO_LAUNCH(colsum_seg_kernel, dim3((N + 31) / 32, M / period), 256, 0, (cudaStream_t)stream, out, ldo, A, lda, N, period);
+    TACO_LAUNCH_CHECK();
+    return 0;
+}
+
+int taco_guided_attention_partial_count(int B, int T) { return (B > 0 && T > 0) ? B * T : 0; }
+
+int taco_guided_attention(float* dscore, float* loss, const float* align, const int32_t* text_length,
+                          const int32_t* speech_steps, int B, int T, int Tx, float g, float lam, float* partial_ws,
+                          void* stream) {
+    TACO_CHECK(dscore && loss && align && text_length && speech_steps && partial_ws, "taco_guided_attention: NULL");
+    TACO_CHECK(B >= 1 && T >= 1 && Tx >= 1 && Tx <= 256 && (int64_t)B * T <= INT32_MAX,
+               "taco_guided_attention: bad sizes (B=%d, T=%d, Tx=%d; Tx <= 256)", B, T, Tx);
+    TACO_CHECK(g > 0.f && g <= 3.0e38f, "taco_guided_attention: g=%g must be finite and positive", (double)g);
+    TACO_CHECK(lam >= 0.f && lam <= 3.0e38f, "taco_guided_attention: lam=%g must be finite and >= 0", (double)lam);
+    const int64_t rows = (int64_t)B * T;
+    // the grid only sets how rows are dealt to warps: every row's arithmetic, and the reduction, are independent of it
+    int blocks = (int)((rows + GA_WARPS - 1) / GA_WARPS);
+    if (blocks > TACO_SMS * 8) blocks = TACO_SMS * 8;
+    const float inv_2g2 = (float)(0.5 / ((double)g * (double)g));
+    TACO_LAUNCH(guided_attention_kernel, blocks, 256, 0, (cudaStream_t)stream, dscore, partial_ws, align, text_length,
+                speech_steps, B, T, Tx, inv_2g2, lam);
+    TACO_LAUNCH_CHECK();
+    TACO_LAUNCH(guided_attention_sum_kernel, 1, 256, 0, (cudaStream_t)stream, partial_ws, rows, (double)lam, loss);
     TACO_LAUNCH_CHECK();
     return 0;
 }

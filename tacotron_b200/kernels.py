@@ -334,11 +334,37 @@ def decoder_bwd(a):
     if a.get("DH0") is not None:                             # out: d(loss)/d(h_i(-1)) [3][B][256]
         assert a["DH0"].is_contiguous() and a["DH0"].is_cuda and tuple(a["DH0"].shape) == (3, B, 256)
         d.DH0 = a["DH0"].data_ptr()
+    if a.get("dscore_add") is not None:                      # [B][T][Tx] added to every step's dscore (guided attention)
+        assert a["dscore_add"].is_contiguous() and a["dscore_add"].is_cuda and a["dscore_add"].shape == a["align"].shape
+        d.dscore_add = a["dscore_add"].data_ptr()
     ws = torch.empty(L.lib().taco_decoder_bwd_workspace_bytes() // 4, dtype=torch.float32, device=a["dy_ext"].device)
     d.workspace = ws.data_ptr()
     d.max_ctas = int(a.get("max_ctas") or 0)                 # CTA budget, 0 = the device's capacity
     L.check(L.lib().taco_decoder_bwd(C.byref(d), _st()), "taco_decoder_bwd")
     a["_ws"] = ws                                            # keep the scratch alive until the stream has consumed it
+
+
+def guided_attention(dscore, loss, align, text_length, speech_steps, g, lam, partial=None):
+    """Guided attention loss (include/taco_b200.h taco_guided_attention; tests/mirror_kernels_guided.py): dscore fp32
+    [B,T,Tx] <- d(loss)/d(attention scores), loss fp32 [1] <- lam * sum align * W, for the alignments align [B,T,Tx],
+    text_length and speech_steps int32 [B].  partial: fp32 scratch of taco_guided_attention_partial_count(B, T) floats
+    (allocated when None)."""
+    B, T, Tx = align.shape
+    _f32c(align, "guided_attention align"); _f32c(dscore, "guided_attention dscore"); _f32c(loss, "guided_attention loss")
+    _cuda_c(text_length, torch.int32, "guided_attention text_length")
+    _cuda_c(speech_steps, torch.int32, "guided_attention speech_steps")
+    if dscore.shape != align.shape or loss.numel() != 1 or text_length.shape != (B,) or speech_steps.shape != (B,):
+        raise L.TacoError(f"guided_attention: align [B,T,Tx] = {tuple(align.shape)} needs dscore of that shape, a 1-element "
+                          f"loss and [B] lengths, got {tuple(dscore.shape)}, {tuple(loss.shape)}, "
+                          f"{tuple(text_length.shape)}, {tuple(speech_steps.shape)}")
+    n = L.lib().taco_guided_attention_partial_count(B, T)
+    if partial is None:
+        partial = torch.empty(n, dtype=torch.float32, device=align.device)
+    _f32c(partial, "guided_attention partial")
+    if partial.numel() < n:
+        raise L.TacoError(f"guided_attention: partial holds {partial.numel()} floats, needs {n}")
+    L.check(L.lib().taco_guided_attention(_p(dscore), _p(loss), _p(align), _p(text_length), _p(speech_steps), B, T, Tx,
+                                          float(g), float(lam), _p(partial), _st()), "taco_guided_attention")
 
 
 def decoder_capacity():

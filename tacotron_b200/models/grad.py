@@ -378,6 +378,8 @@ def decoder_bwd(K, P, G, S, cfg, dY_ext):
     if h0 is not None:
         a["H0"] = [h0[i] for i in range(3)]
         a["DH0"] = K.empty((3, B, U), like)
+    if S.get("dec/dscore_ga") is not None:                # guided attention loss: its d(loss)/d(score), added to the
+        a["dscore_add"] = S["dec/dscore_ga"]              # softmax backward's dscore of every step
     K.decoder_bwd(a)
     if "_capture" in S:                                   # tests: expose the serial kernel's arguments and outputs
         S["_capture"]["decoder_bwd"] = a
@@ -449,7 +451,8 @@ def decoder_speaker_bwd(K, P, G, S, DZ0, DH0):
 # whole model: reverse of Tacotron.inference + add_loss_op (models/tacotron.py:107-165)
 # ------------------------------------------------------------------------------------------------------------
 def model_bwd(K, P, G, S, cfg):
-    """Accumulates d(loss)/d(param) into G for loss = sum|seq2seq_output - mel| + sum|output - stft|."""
+    """Accumulates d(loss)/d(param) into G for loss = sum|seq2seq_output - mel| + sum|output - stft|, plus the guided
+    attention loss when S['dec/dscore_ga'] holds its gradient with respect to the attention scores."""
     y, out = S["dec/y"], S["post/out"]
     B, T, OUT = y.shape
     mf, r = cfg.mel_features, cfg.r

@@ -6,6 +6,8 @@ written kernels; the attribute names the reference drivers fetch (``seq2seq_outp
 """
 from __future__ import annotations
 
+import math
+
 import torch
 
 from .. import _lib as L
@@ -55,6 +57,10 @@ class Config(object):
     max_ctas = None
     # multi-speaker models: condition the decoder on the speaker too (initial attention vector and GRU states, DESIGN.md §7)
     speaker_decoder = False
+    # guided attention loss (Tachibana et al. 2017, arXiv:1710.08969): lambda (0 = off) and the width g of the band around
+    # the text-speech diagonal outside which attention weight is penalised.  Training only; needs inputs['speech_steps'].
+    guided_attention = 0.0
+    guided_attention_g = 0.2
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -84,6 +90,7 @@ class Tacotron(object):
         self.lr = config.init_lr
         self.global_step = 0
         self.seq2seq_output = self.output = self.alignments = self.loss = None
+        self.guided_attention_loss = None
         self.step_ns = None
         self.section_wait = None
         self.last_graph_kernels = 0                # kernels inside the CUDA graphs replayed by the last call
@@ -352,10 +359,21 @@ class Tacotron(object):
         from .. import kernels as K
         self.add_train_op()
         lr = self.lr if lr is None else lr
+        lam = self._guided_attention_lambda(inputs)
         S = {}
         with ops.saving(S):
             self.seq2seq_output, self.output = self.inference(inputs, True, **kw)
         self.loss = self.add_loss_op(self.seq2seq_output, self.output, inputs["mel"], inputs["stft"])
+        if lam > 0:                                # + guided attention loss; its score gradient goes to the decoder backward
+            align = S["dec/align"]
+            dscore = torch.empty_like(align)
+            ga = self.runtime.buf("loss/ga", (1,))
+            part = self.runtime.buf("loss/ga_partial", (L.lib().taco_guided_attention_partial_count(*align.shape[:2]),))
+            K.guided_attention(dscore, ga, align, inputs["text_length"], inputs["speech_steps"],
+                               self.config.guided_attention_g, lam, part)
+            S["dec/dscore_ga"] = dscore
+            self.guided_attention_loss = ga[0]
+            self.loss = self.loss + ga[0]
         S.update(text=inputs["text"], text_length=inputs["text_length"], mel=inputs["mel"], stft=inputs["stft"])
         if self.config.num_speakers > 1:
             S["speaker"] = inputs["speaker"]
@@ -368,6 +386,30 @@ class Tacotron(object):
         self.store.version += 1                    # derived kernel-layout buffers are refreshed on the next forward
         self.global_step += 1
         return self.loss
+
+    def _guided_attention_lambda(self, inputs):
+        """lambda of the guided attention loss (0.0 = off), after checking the settings and inputs['speech_steps'] (int32
+        [B]: the voiced decoder steps T_b of each target, in [1, T]; the range check reads them to the host once)"""
+        lam = float(getattr(self.config, "guided_attention", 0.0) or 0.0)
+        g = float(getattr(self.config, "guided_attention_g", 0.2))
+        if not (math.isfinite(lam) and lam >= 0.0):
+            raise ValueError(f"Config.guided_attention = {lam}: the loss weight must be finite and >= 0 (0 = off)")
+        if lam == 0.0:
+            return 0.0
+        if not (math.isfinite(g) and g > 0.0):
+            raise ValueError(f"Config.guided_attention_g = {g}: the band width must be finite and > 0")
+        steps = inputs.get("speech_steps")
+        if steps is None:
+            raise ValueError("Config.guided_attention > 0 needs inputs['speech_steps'] (int32 [B]): the voiced decoder steps "
+                             "of each target, e.g. audio.speech_frames(inputs['stft'], r, stft_mean, stft_std) // r")
+        B, T = inputs["mel"].shape[:2]
+        if not (steps.dtype == torch.int32 and steps.is_cuda and steps.is_contiguous() and tuple(steps.shape) == (B,)):
+            raise ValueError(f"inputs['speech_steps'] must be a contiguous int32 CUDA tensor of shape [{B}], got "
+                             f"{steps.dtype} {steps.device} {tuple(steps.shape)}")
+        lo, hi = torch.stack([steps.min(), steps.max()]).tolist()
+        if lo < 1 or hi > T:
+            raise ValueError(f"inputs['speech_steps'] must lie in [1, {T}] (the decoder steps of the batch), got [{lo}, {hi}]")
+        return lam
 
     # -- the eager stand-in for sess.run([...]) ---------------------------------------------------
     def __call__(self, inputs, **kw):

@@ -40,6 +40,7 @@ from .tf_checkpoint import _field, _put_varint, crc32c, mask_crc
 
 HISTOGRAM_TAGS = ("encoder/pre_net_out", "decoder/seq2seq_output", "post-process/output")     # tacotron.py:129,139,152
 SCALAR_TAGS = ("seq2seq_loss", "output_loss", "loss", "cap_grads/global_gradient_norm")       # :162-164, :181
+GUIDED_ATTENTION_TAG = "guided_attention_loss"         # (new) Config.guided_attention > 0: the guided attention loss
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -265,28 +266,35 @@ class TrainSummaries:
     ``enqueue`` (after the step's update, before its one host sync) bins the three histogrammed tensors with
     ``kernels.histogram`` and queues copies of their results and of the four scalars into pinned buffers; ``collect``
     (after the sync) takes them; ``write_pending`` encodes them -- the driver calls it once the NEXT step is enqueued, so the
-    encoding and the CRCs run while the GPU computes."""
+    encoding and the CRCs run while the GPU computes.  guided_attention=True adds the scalar GUIDED_ATTENTION_TAG, the
+    fourth loss ``enqueue`` then takes."""
 
-    def __init__(self, logdir, device, log=print):
+    def __init__(self, logdir, device, log=print, guided_attention=False):
         import torch
         self.writer = EventWriter(logdir)
         self.limits = histogram_limits()
         self.limits_d = torch.from_numpy(self.limits).to(device)
         self.res = torch.empty((len(HISTOGRAM_TAGS), len(self.limits) + 5), dtype=torch.int64, device=device)
         self.res_h = torch.empty(self.res.shape, dtype=torch.int64, pin_memory=True)
-        self.scal_h = torch.empty(len(SCALAR_TAGS), dtype=torch.float32, pin_memory=True)
+        self.guided_attention = bool(guided_attention)
+        self.scal_h = torch.empty(len(SCALAR_TAGS) + self.guided_attention, dtype=torch.float32, pin_memory=True)
         self.log = log
         self._queued = None
         self._pending = []
 
     def enqueue(self, step, tensors, losses, grad_sumsq):
-        """tensors: the pre-net output, seq2seq_output and output; losses: device [loss, seq2seq loss, output loss]"""
+        """tensors: the pre-net output, seq2seq_output and output; losses: device [loss, seq2seq loss, output loss] (and the
+        guided attention loss fourth, when the summaries were built with guided_attention=True)"""
         from . import kernels as K
+        if len(losses) != 3 + self.guided_attention:
+            raise ValueError(f"TrainSummaries.enqueue: {len(losses)} losses, expected {3 + self.guided_attention}")
         for i, t in enumerate(tensors):
             K.histogram(self.res[i], t, self.limits_d)
         self.res_h.copy_(self.res, non_blocking=True)
-        self.scal_h[:3].copy_(losses, non_blocking=True)
-        self.scal_h[3:].copy_(grad_sumsq.reshape(1), non_blocking=True)
+        self.scal_h[:3].copy_(losses[:3], non_blocking=True)
+        self.scal_h[3:4].copy_(grad_sumsq.reshape(1), non_blocking=True)
+        if self.guided_attention:
+            self.scal_h[4:].copy_(losses[3:], non_blocking=True)
         self._queued = step
 
     def collect(self):
@@ -299,6 +307,8 @@ class TrainSummaries:
             vals = histogram_values(res, self.limits, self.log)
             norm = np.sqrt(np.float32(scal[3]))                              # tf.global_norm, before clipping
             vals += [scalar_value(t, v) for t, v in zip(SCALAR_TAGS, (scal[1], scal[2], scal[0], norm))]
+            if self.guided_attention:
+                vals.append(scalar_value(GUIDED_ATTENTION_TAG, scal[4]))
             self.writer.add(step, vals)
         self._pending = []
 

@@ -14,6 +14,7 @@ batches of 32 and all-reduce the flat gradient bucket inside ``model.train_step`
 from __future__ import annotations
 
 import argparse
+import math
 import os
 import sys
 
@@ -34,7 +35,9 @@ def write_wav(path, wave, sr):
 def train(model_cls, config, num_steps=1000000, log=print, save_every=SAVE_EVERY, summary_dir=None, summary_every=1):
     """summary_dir: write TensorBoard summaries there (tacotron_b200/summary.py): the losses, the global gradient norm and
     the histograms of the pre-net output, seq2seq_output and output every `summary_every` steps, the two clips and the
-    attention image at every save step.  The histograms are rank 0's batch."""
+    attention image at every save step.  The histograms are rank 0's batch.
+    config.guided_attention > 0 adds the guided attention loss: each batch gets inputs['speech_steps'], the voiced decoder
+    steps of its targets (audio.speech_frames), and the loss is summarised and logged as a fourth loss."""
     from . import audio, checkpoint, data_input
     from .utils import dist as D
     world, rank, local = D.world()
@@ -66,16 +69,20 @@ def train(model_cls, config, num_steps=1000000, log=print, save_every=SAVE_EVERY
     lr = model.config.init_lr                                                            # :60
     annealing_rate = model.config.annealing_rate                                         # :61
     # summaries (train.py:41,64-75): rank 0 writes; every rank takes part in the one all-reduce of the three losses
+    guided = float(getattr(config, "guided_attention", 0.0) or 0.0) > 0
     summaries = None
     if summary_dir is not None and rank == 0:
         from . import summary
-        summaries = summary.TrainSummaries(summary_dir, torch.device("cuda", local), log)
+        summaries = summary.TrainSummaries(summary_dir, torch.device("cuda", local), log, guided_attention=guided)
     try:
         for _ in range(num_steps):                                                       # :63
             inputs = next(batches)
+            if guided:             # T_b of the guided attention loss: where each target's speech ends, in decoder steps
+                inputs["speech_steps"] = audio.speech_frames(inputs["stft"], config.r, mean_d, std_d) // config.r
             loss_t = train_op(inputs, lr).reshape(1).clone()                             # :64-73
-            if summary_dir is not None:
-                loss_t = torch.stack([model.loss, model.seq2seq_loss, model.output_loss])
+            if summary_dir is not None or guided:
+                loss_t = torch.stack([model.loss, model.seq2seq_loss, model.output_loss]
+                                     + ([model.guided_attention_loss] if guided else []))
             if world > 1:                  # every rank must take the same branch below (a rank that leaves alone hangs the
                 torch.distributed.all_reduce(loss_t)   # next gradient all-reduce): the guard and the log use the global loss
             global_step = model.global_step
@@ -88,7 +95,8 @@ def train(model_cls, config, num_steps=1000000, log=print, save_every=SAVE_EVERY
             if summaries is not None:
                 summaries.collect()
             if rank == 0 and global_step % 100 == 0:
-                log(f"step {global_step} loss {loss:.1f} lr {lr:.3g} grad-norm {float(model.grad_sumsq.sqrt()):.1f}")
+                ga = f" guided-attention {float(loss_t[3]):.4g}" if guided else ""
+                log(f"step {global_step} loss {loss:.1f}{ga} lr {lr:.3g} grad-norm {float(model.grad_sumsq.sqrt()):.1f}")
             if loss > 1e8 and global_step > 500:                                         # :75-77 detect gradient explosion
                 log("loss exploded")
                 break
@@ -113,7 +121,8 @@ def train(model_cls, config, num_steps=1000000, log=print, save_every=SAVE_EVERY
     return model
 
 
-def main(argv=None):
+def config_from_args(argv=None):
+    """(Config, args) of the command line"""
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", "--train-set", default="nancy")
     parser.add_argument("-d", "--debug", type=bool, default=False)
@@ -126,14 +135,31 @@ def main(argv=None):
     parser.add_argument("--speaker-decoder", action="store_true",
                         help="multi-speaker data: condition the decoder on the speaker too (initial attention vector and "
                              "GRU states)")
+    parser.add_argument("--guided-attention", type=float, default=0.0, metavar="LAMBDA",
+                        help="weight of the guided attention loss (Tachibana et al. 2017), a sum like the two L1 losses; "
+                             "0 = off (default).  No value has been validated: see README")
+    parser.add_argument("--guided-attention-g", type=float, default=0.2, metavar="G",
+                        help="width of the guided attention band around the text-speech diagonal (default 0.2)")
     args = parser.parse_args(argv)
-    from .models.tacotron import Config, Tacotron
+    if not (math.isfinite(args.guided_attention) and args.guided_attention >= 0):
+        parser.error(f"--guided-attention {args.guided_attention}: must be finite and >= 0")
+    if not (math.isfinite(args.guided_attention_g) and args.guided_attention_g > 0):
+        parser.error(f"--guided-attention-g {args.guided_attention_g}: must be finite and > 0")
+    from .models.tacotron import Config
     config = Config()
     config.data_path = "data/%s/" % args.train_set                                       # train.py:108
     config.restore = args.restore
     config.save_path = "debug" if args.debug else "%s/tacotron" % args.train_set         # :110-113
     config.max_ctas = args.max_ctas
     config.speaker_decoder = args.speaker_decoder
+    config.guided_attention = args.guided_attention
+    config.guided_attention_g = args.guided_attention_g
+    return config, args
+
+
+def main(argv=None):
+    from .models.tacotron import Tacotron
+    config, args = config_from_args(argv)
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "train") if args.summaries else None     # train.py:41
     train(Tacotron, config, num_steps=args.steps, summary_dir=summary_dir, summary_every=args.summary_every)
