@@ -145,6 +145,38 @@ int taco_bigru_fwd_h0(const float* xp, const float* Wg_h_fw, const float* Wc_h_f
                       float* out, int B, int T, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * taco_highway_stack_fwd -- the pointwise tail of a CBHG at inference (models/ops.py:27-46,118-128) in ONE kernel:
+ *   h = X (C == 128), or X.Wd + bd (width-fixing dense, C != 128, ops.py:29-30)
+ *   L times: h = relu(h.WH + bH) * sig(h.WT + bT) + h * (1 - sig(h.WT + bT))          (highway, ops.py:32-45)
+ *   Y = h.Wx + bx: the bi-GRU input products xp, in taco_bigru_fwd's layout           (ops.py:118-128)
+ * over M flat rows (every layer is a dense, so utterance boundaries do not matter).  Only Y is written; the
+ * activations between layers stay on chip.  TACO_IMPL_TC3 only.  Weights are the buffers taco_pack_weight_x3 makes
+ * for the unfused route (hi rows [0,N), lo rows [N,2N)): Wd_p N = 128, hw_p[l] = [WH | WT] with N = 256, xp_p N = 768.
+ * Each output element sees the same operations in the same order as that of the unfused sequence
+ * (taco_linear_fwd dense + L x TACO_EPI_HIGHWAY + dense 768), so the results are bit-identical to it.
+ * ------------------------------------------------------------------------------------------ */
+#define TACO_HIGHWAY_STACK_MAX 4
+typedef struct taco_highway_stack_desc {
+    const float*   X;        /* [M][ldx], C valid channels                                    */
+    int64_t        ldx;
+    int32_t        M, C;     /* 1 <= C <= 128                                                 */
+    const float*   Wd_p;     /* packed [2*128][ldwd] (C != 128), NULL when C == 128           */
+    int64_t        ldwd;
+    const float*   bd;       /* [128] (C != 128)                                              */
+    int32_t        L;        /* highway layers, 1..TACO_HIGHWAY_STACK_MAX                     */
+    const float*   hw_p[TACO_HIGHWAY_STACK_MAX];   /* packed [2*256][ldhw]                    */
+    int64_t        ldhw;
+    const float*   hw_b[TACO_HIGHWAY_STACK_MAX];   /* [bH | bT] (256)                         */
+    const float*   xp_p;     /* packed [2*768][ldxp]                                          */
+    int64_t        ldxp;
+    const float*   xp_b;     /* [768]                                                         */
+    float*         Y;        /* [M][ldy], ldy >= 768                                          */
+    int64_t        ldy;
+    int32_t        impl;     /* TACO_IMPL_TC3                                                 */
+} taco_highway_stack_desc;
+int taco_highway_stack_fwd(const taco_highway_stack_desc* d, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Decoder: tacotron.py:46-105 create_decoder + :136-138 dynamic_decode, i.e. per step
  *   pre_net(last frame) ++ attention -> InputProjection -> 3x GRUCell(256) -> Residual ->
  *   OutputProjection(80r) -> BahdanauAttention(query = cell output) -> attention layer.

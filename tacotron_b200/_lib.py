@@ -36,6 +36,21 @@ class LinearDesc(C.Structure):
     ]
 
 
+HIGHWAY_STACK_MAX = 4
+
+
+class HighwayStackDesc(C.Structure):
+    _fields_ = [
+        ("X", C.c_void_p), ("ldx", C.c_int64), ("M", C.c_int32), ("C", C.c_int32),
+        ("Wd_p", C.c_void_p), ("ldwd", C.c_int64), ("bd", C.c_void_p),
+        ("L", C.c_int32),
+        ("hw_p", C.c_void_p * HIGHWAY_STACK_MAX), ("ldhw", C.c_int64), ("hw_b", C.c_void_p * HIGHWAY_STACK_MAX),
+        ("xp_p", C.c_void_p), ("ldxp", C.c_int64), ("xp_b", C.c_void_p),
+        ("Y", C.c_void_p), ("ldy", C.c_int64),
+        ("impl", C.c_int32),
+    ]
+
+
 class DecoderWeights(C.Structure):
     _fields_ = [
         ("pre_W1", C.c_void_p), ("pre_b1", C.c_void_p), ("pre_W2", C.c_void_p), ("pre_b2", C.c_void_p),
@@ -96,7 +111,7 @@ _lib = None
 # every symbol include/taco_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "taco_last_error", "taco_version", "taco_device_info", "taco_linear_fwd", "taco_linear_route", "taco_pack_weight",
-    "taco_pack_weight_x3",
+    "taco_pack_weight_x3", "taco_highway_stack_fwd",
     "taco_maxpool_fwd", "taco_gather_rows", "taco_mask_rows", "taco_bigru_fwd", "taco_bigru_fwd_h0",
     "taco_decoder_packed_bytes", "taco_decoder_workspace_bytes", "taco_decoder_pack", "taco_decoder_fwd",
     "taco_decoder_capacity",
@@ -141,6 +156,7 @@ def lib():
     L.taco_pack_weight.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
     L.taco_conv_dw.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64] + [C.c_int32] * 6 + [C.c_void_p]
     L.taco_pack_weight_x3.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    L.taco_highway_stack_fwd.argtypes = [C.POINTER(HighwayStackDesc), C.c_void_p]
     L.taco_maxpool_fwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     L.taco_gather_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_float,
                                    C.c_void_p, C.c_void_p]

@@ -20,6 +20,7 @@ int taco_pack_weight_impl(const float* W, int taps, int C, int N, float* dst, in
 int taco_pack_weight_x3_impl(const float* W, int taps, int C, int N, float* dst_hi, float* dst_lo, int64_t ld_dst, cudaStream_t st);
 int taco_conv_dw_tc_impl(float* dW, int64_t ldw, int64_t tap_stride, const float* X, int64_t ldx, const float* dZ, int64_t lddz,
                          int B, int T, int C, int N, int taps, int tap0, cudaStream_t st);
+int taco_highway_stack(const taco_highway_stack_desc* d, cudaStream_t st);
 
 namespace {
 
@@ -172,6 +173,10 @@ int taco_linear_route(const taco_linear_desc* d, int* bn, int* stages, int* mode
     if (direct) *direct = r.direct;
     if (tile_stride) *tile_stride = r.tile_stride;
     return 0;
+}
+
+int taco_highway_stack_fwd(const taco_highway_stack_desc* d, void* stream) {
+    return taco_highway_stack(d, (cudaStream_t)stream);
 }
 
 int taco_pack_weight_x3(const float* W, int taps, int C, int N, float* dst_hi, float* dst_lo, int64_t ld_dst, void* stream) {

@@ -1,5 +1,5 @@
-// gemm_tc.cu -- TMA + wgmma implementation of taco_linear_fwd (TACO_IMPL_TC / TACO_IMPL_TC3) and of the tensor-core
-// weight gradient taco_conv_dw, sm_90a.
+// gemm_tc.cu -- TMA + wgmma implementation of taco_linear_fwd (TACO_IMPL_TC / TACO_IMPL_TC3), of the tensor-core
+// weight gradient taco_conv_dw and of the fused CBHG highway stack taco_highway_stack_fwd, sm_90a.
 //
 // One kernel serves every feed-forward contraction of the model (conv bank as ONE grouped
 // implicit GEMM, conv projections, highway, GRU input products, attention memory layer,
@@ -679,6 +679,248 @@ __global__ void __launch_bounds__(DW_THREADS, 1) dw_tc_kernel(const __grid_const
     }
 }
 
+// =====================================================================================================================
+// taco_highway_stack_fwd: the pointwise tail of a CBHG inference (width-fixing dense, the highway layers, the bi-GRU
+// input products) as ONE kernel, 3xTF32 (TACO_IMPL_TC3) only.
+//
+// Every layer of that chain is a dense (taps = 1), so a tile of flat rows (utterance boundaries do not matter) can run
+// the whole chain without its activations leaving the SM:
+//  * one CTA per 128-row tile: TMA loads the input rows once over a 2-D map of the flat rows, as 32-channel k-blocks in
+//    the 128B-swizzled K-major layout the X3 A-fragment reader of gemm_tc_kernel reads (rows past M and channels past C are
+//    zero-filled: C = 80 in the post-net is padded to 96);
+//  * the activation tile (128 rows x 128 channels, 64 KB) stays in shared memory between layers, in two buffers: a
+//    highway layer's carry x is its own input tile, so each layer reads one buffer and writes the other;
+//  * the weights stream through a 3-deep TMA ring from the packed hi / lo buffers of taco_pack_weight_x3, one stage =
+//    the hi and lo halves of 128 output columns x one k-block (32 KB).  The ring runs through the whole chain in one
+//    order (layer, 128-column chunk, k-block), so the next layer's weights load under the current layer's epilogue;
+//  * warpgroup w multiplies rows [64w, 64w+64) with wgmma m64n128k8 exactly as gemm_tc_kernel<.., X3 = true> does
+//    (same rn_tf32 hi / lo split of A, same lo.hi + hi.lo + hi.hi order per k8 step, k-blocks in order), and the
+//    epilogue runs on the accumulator fragments in registers with the same expressions as that kernel's register-direct
+//    epilogue.  Each output element therefore sees the same operations in the same order as on the unfused route, and
+//    the result is bit-identical to it;
+//  * a warp's A fragments and its epilogue cover the same 16 rows, so a layer's output is ready for the next layer
+//    after a __syncwarp: the two warpgroups share only the weight ring;
+//  * only xp (+ its bias) is written to HBM.  When there are fewer tiles than SMs (the encoder: 32 utterances x 128
+//    characters), grid.y splits the 768 xp columns: each CTA of a tile repeats the (cheap, otherwise idle-SM) highway
+//    layers and writes its share of xp.
+// =====================================================================================================================
+
+constexpr int HS_BM = 128;
+constexpr int HS_BK = 32;                                  // floats: one 128-byte swizzle row
+constexpr int HS_THREADS = 256;                            // two warpgroups
+constexpr int HS_STAGES = 3;
+constexpr int HS_TILE_BYTES = HS_BM * HS_BK * 4;           // 16 KB: 128 rows (or 128 weight columns) x one k-block
+constexpr int HS_ACT_BYTES = 4 * HS_TILE_BYTES;            // 128 rows x 128 channels
+constexpr int HS_STAGE_BYTES = 2 * HS_TILE_BYTES;          // weight hi | lo
+constexpr int HS_RING_OFFSET = 2 * HS_ACT_BYTES;
+constexpr int HS_BAR_OFFSET = HS_RING_OFFSET + HS_STAGES * HS_STAGE_BYTES;
+constexpr int HS_SMEM = HS_BAR_OFFSET + 128 + 1024;        // barriers + alignment slack
+static_assert(HS_SMEM <= 227 * 1024, "shared memory per block exceeds 227 KB");
+constexpr int HS_XP_N = 768;
+constexpr int HS_MAX_LAYERS = TACO_HIGHWAY_STACK_MAX + 2;  // width-fixing dense + highway layers + xp
+
+struct HsMaps {
+    CUtensorMap x;                       // input rows [M][C], box {32 ch, 128 rows}
+    CUtensorMap w[HS_MAX_LAYERS];        // packed weights of each layer, box {32 k, 128 output columns}
+};
+
+struct HsArgs {
+    int M;
+    int nlayers;                         // (dense) + highway layers + xp
+    int dense;                           // 1: layer 0 is the width-fixing dense (C != 128)
+    int kin;                             // k-blocks of layer 0 (round_up(C, 32) / 32)
+    int xp_chunks;                       // 128-column chunks of xp per CTA (6 / grid.y)
+    int total_items;                     // weight stages the CTA consumes
+    int lo_row0[HS_MAX_LAYERS];          // first row of the lo half in each packed buffer (= the layer's N)
+    const float* bias[HS_MAX_LAYERS];    // dense [128], highway [bH | bT] (256), xp [768]
+    float* Y;                            // xp [M][ldy]
+    int64_t ldy;
+};
+
+// byte offset of (row r, channel col) in a 128-row activation tile: k-block col/32, 16-byte chunk (col%32)/4 of row r at
+// chunk ((col%32)/4) ^ (r%8) (SWIZZLE_128B)
+__device__ __forceinline__ int act_off(int r, int col) {
+    const int c = col & 31;
+    return (col >> 5) * HS_TILE_BYTES + r * 128 + (((c >> 2) ^ (r & 7)) << 4) + (c & 3) * 4;
+}
+
+__global__ void __launch_bounds__(HS_THREADS, 1) highway_stack_kernel(const __grid_constant__ HsMaps maps, const __grid_constant__ HsArgs a) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* ring = smem + HS_RING_OFFSET;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + HS_BAR_OFFSET);
+    uint64_t* empty_bar = full_bar + HS_STAGES;
+    uint64_t* in_bar = empty_bar + HS_STAGES;
+
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5;
+    const int lane = tid & 31;
+    const int row0 = blockIdx.x * HS_BM;
+    const int xp_chunk0 = blockIdx.y * a.xp_chunks;
+
+    auto nchunks = [&](int l) { return l == a.nlayers - 1 ? a.xp_chunks : (a.dense && l == 0) ? 1 : 2; };
+    auto kblocks = [&](int l) { return l == 0 ? a.kin : 4; };
+
+    // producer cursor (thread 0 only): the next weight stage to load, in consumption order
+    int pl = 0, pch = 0, pkb = 0;
+    auto issue = [&](int it) {
+        const int s = it % HS_STAGES;
+        uint8_t* Bs = ring + s * HS_STAGE_BYTES;
+        const int n0 = ((pl == a.nlayers - 1) ? xp_chunk0 + pch : pch) * 128;
+        mbar_arrive_expect_tx(&full_bar[s], HS_STAGE_BYTES);
+        tma_load_2d(Bs, &maps.w[pl], &full_bar[s], pkb * HS_BK, n0);
+        tma_load_2d(Bs + HS_TILE_BYTES, &maps.w[pl], &full_bar[s], pkb * HS_BK, a.lo_row0[pl] + n0);
+        if (++pkb == kblocks(pl)) {
+            pkb = 0;
+            if (++pch == nchunks(pl)) { pch = 0; ++pl; }
+        }
+    };
+
+    if (tid == 0) {
+        tma_prefetch_desc(&maps.x);
+        for (int s = 0; s < HS_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], HS_THREADS / 32); }
+        mbar_init(in_bar, 1);
+        mbar_fence_init();
+    }
+    __syncthreads();
+    if (tid == 0) {
+        mbar_arrive_expect_tx(in_bar, a.kin * HS_TILE_BYTES);
+        for (int kb = 0; kb < a.kin; ++kb) tma_load_2d(smem + kb * HS_TILE_BYTES, &maps.x, in_bar, kb * HS_BK, row0);
+        for (int it = 0; it < HS_STAGES && it < a.total_items; ++it) issue(it);
+    }
+
+    const int wg = tid >> 7;
+    const int g = lane >> 2, tg = lane & 3;
+    const int frow = wg * 64 + (warp & 3) * 16 + g;       // first tile row of this thread's A / accumulator fragments
+    int it = 0;                                           // weight stage being consumed
+
+    // one 128-column chunk of a layer: d = act_in[rows, 0 : 32 kb) . W[:, chunk], k-blocks in order (gemm_tc_kernel X3)
+    auto mma_chunk = [&](float (&d)[64], const uint8_t* act_in, int kb_n) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d[i] = 0.f;
+        for (int kb = 0; kb < kb_n; ++kb, ++it) {
+            const int s = it % HS_STAGES;
+            const uint32_t ph = (it / HS_STAGES) & 1;
+            mbar_wait(&full_bar[s], ph);
+            const uint8_t* As = act_in + kb * HS_TILE_BYTES;
+            const uint32_t b_addr = smem_u32(ring + s * HS_STAGE_BYTES);
+            const uint64_t bhi = wgmma_desc_sw128(b_addr);
+            const uint64_t blo = wgmma_desc_sw128(b_addr + HS_TILE_BYTES);
+            uint32_t ah[HS_BK / 8][4], al[HS_BK / 8][4];
+#pragma unroll
+            for (int k = 0; k < HS_BK / 8; ++k) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int r = frow + 8 * (e & 1);
+                    const int c = 8 * k + tg + 4 * (e >> 1);
+                    const float x = *reinterpret_cast<const float*>(As + r * 128 + (((c >> 2) ^ (r & 7)) << 4) + (c & 3) * 4);
+                    const float hv = rn_tf32(x);
+                    ah[k][e] = __float_as_uint(hv);
+                    al[k][e] = __float_as_uint(rn_tf32(x - hv));
+                }
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < HS_BK / 8; ++k) {
+                wgmma_m64n128k8_rs(d, al[k], bhi + (uint64_t)(2 * k));     // lo . hi
+                wgmma_m64n128k8_rs(d, ah[k], blo + (uint64_t)(2 * k));     // hi . lo
+                wgmma_m64n128k8_rs(d, ah[k], bhi + (uint64_t)(2 * k));     // hi . hi
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[s]);           // this warp's products have read the stage
+            if (tid == 0 && it + HS_STAGES < a.total_items) {
+                mbar_wait(&empty_bar[s], ph);
+                issue(it + HS_STAGES);
+            }
+        }
+    };
+
+    mbar_wait(in_bar, 0);
+    uint8_t* act_in = smem;
+    uint8_t* act_out = smem + HS_ACT_BYTES;
+    float acc[64], acc2[64];
+    // accumulator fragment i = 4j + e of this thread: row frow + 8 (e >> 1), column 8j + 2 tg + (e & 1) of the chunk
+    for (int l = 0; l < a.nlayers; ++l) {
+        const float* bias = a.bias[l];
+        if (l == a.nlayers - 1) {
+            // ---- bi-GRU input products: xp = h . Wx + bx, the only output that leaves the SM ----
+            for (int ch = 0; ch < a.xp_chunks; ++ch) {
+                mma_chunk(acc, act_in, kblocks(l));
+                const int n0 = (xp_chunk0 + ch) * 128;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int grow = row0 + frow + 8 * h;
+                    if (grow < a.M) {
+                        float* yp = a.Y + (int64_t)grow * a.ldy + n0 + 2 * tg;
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            const float b0 = __ldg(bias + n0 + 8 * j + 2 * tg), b1 = __ldg(bias + n0 + 8 * j + 2 * tg + 1);
+                            *reinterpret_cast<float2*>(yp + 8 * j) =
+                                make_float2(fmaf(acc[4 * j + 2 * h] + b0, 1.f, 0.f), fmaf(acc[4 * j + 2 * h + 1] + b1, 1.f, 0.f));
+                        }
+                    }
+                }
+            }
+        } else if (a.dense && l == 0) {
+            // ---- width-fixing dense (models/ops.py:29-30): y = x . Wd + bd ----
+            mma_chunk(acc, act_in, kblocks(l));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = frow + 8 * h;
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int col = 8 * j + 2 * tg;
+                    const float b0 = __ldg(bias + col), b1 = __ldg(bias + col + 1);
+                    *reinterpret_cast<float2*>(act_out + act_off(r, col)) =
+                        make_float2(fmaf(acc[4 * j + 2 * h] + b0, 1.f, 0.f), fmaf(acc[4 * j + 2 * h + 1] + b1, 1.f, 0.f));
+                }
+            }
+            __syncwarp();
+            uint8_t* t = act_in; act_in = act_out; act_out = t;
+        } else {
+            // ---- highway (models/ops.py:32-45): H = relu(x.WH + bH), T = sigmoid(x.WT + bT), y = H T + x (1 - T) ----
+            mma_chunk(acc, act_in, kblocks(l));
+            mma_chunk(acc2, act_in, kblocks(l));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = frow + 8 * h;
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int col = 8 * j + 2 * tg;
+                    const float2 x = *reinterpret_cast<const float2*>(act_in + act_off(r, col));
+                    const float xs[2] = {x.x, x.y};
+                    float y[2];
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {
+                        const float H = fmaxf(acc[4 * j + 2 * h + k] + __ldg(bias + col + k), 0.f);
+                        const float Tg = sigmoidf_acc(acc2[4 * j + 2 * h + k] + __ldg(bias + 128 + col + k));
+                        y[k] = H * Tg + xs[k] * (1.0f - Tg);
+                    }
+                    *reinterpret_cast<float2*>(act_out + act_off(r, col)) = make_float2(y[0], y[1]);
+                }
+            }
+            __syncwarp();
+            uint8_t* t = act_in; act_in = act_out; act_out = t;
+        }
+    }
+}
+
+// 2-D fp32 map [rows][cols] (row stride ld floats), box {32 columns, 128 rows}, 128-byte swizzle
+int encode_2d(EncodeTiledFn enc, CUtensorMap* m, const float* base, int64_t cols, int64_t rows, int64_t ld, const char* what) {
+    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+    cuuint32_t box[2] = {HS_BK, HS_BM};
+    cuuint32_t es[2] = {1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, es,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    TACO_CHECK(r == CUDA_SUCCESS, "taco_highway_stack_fwd: cuTensorMapEncodeTiled(%s) failed: %d (cols=%lld rows=%lld ld=%lld)", what,
+               (int)r, (long long)cols, (long long)rows, (long long)ld);
+    return 0;
+}
+
 template <int BN, int STAGES, int MODE, bool X3 = false>
 int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, dim3 grid, cudaStream_t st) {
     using L = SmemLayout<BN, STAGES, X3>;
@@ -869,4 +1111,75 @@ int taco_linear_tc(const taco_linear_desc* d, cudaStream_t st) {
     if (highway) return launch_tc<256, 2, 1>(tmA, tmB, a, grid, st);
     if (r.stages == 2) return launch_tc<128, 2, 0>(tmA, tmB, a, grid, st);
     return launch_tc<128, 3, 0>(tmA, tmB, a, grid, st);
+}
+
+// the checks of a descriptor that need no device
+static int taco_highway_stack_check(const taco_highway_stack_desc* d) {
+    TACO_CHECK(d != nullptr, "taco_highway_stack_fwd: NULL descriptor");
+    TACO_CHECK(d->impl == TACO_IMPL_TC3, "taco_highway_stack_fwd: only TACO_IMPL_TC3 (fp32x3) is implemented (impl %d)", d->impl);
+    TACO_CHECK(d->M >= 0 && d->C >= 1 && d->C <= 128, "taco_highway_stack_fwd: bad sizes M=%d C=%d (1 <= C <= 128)", d->M, d->C);
+    TACO_CHECK(d->L >= 1 && d->L <= TACO_HIGHWAY_STACK_MAX, "taco_highway_stack_fwd: L=%d highway layers (1..%d)", d->L,
+               TACO_HIGHWAY_STACK_MAX);
+    TACO_CHECK(d->X && d->Y && d->xp_p && d->xp_b, "taco_highway_stack_fwd: X, Y, xp_p or xp_b is NULL");
+    TACO_CHECK((d->C == 128) == (d->Wd_p == nullptr), "taco_highway_stack_fwd: the width-fixing dense (Wd_p, bd) is used iff C != 128");
+    TACO_CHECK(d->C == 128 || d->bd, "taco_highway_stack_fwd: bd is NULL");
+    for (int l = 0; l < d->L; ++l)
+        TACO_CHECK(d->hw_p[l] && d->hw_b[l] && taco_aligned16(d->hw_p[l]), "taco_highway_stack_fwd: highway layer %d: NULL or unaligned", l);
+    TACO_CHECK(taco_aligned16(d->X) && taco_aligned16(d->xp_p) && taco_aligned16(d->Y) && (!d->Wd_p || taco_aligned16(d->Wd_p)),
+               "taco_highway_stack_fwd: X, Y and the packed weights must be 16-byte aligned");
+    const int Cpad = (d->C + 31) / 32 * 32;
+    TACO_CHECK(d->ldx >= d->C && (d->ldx % 4) == 0, "taco_highway_stack_fwd: ldx %lld (>= C, multiple of 4)", (long long)d->ldx);
+    TACO_CHECK(d->ldy >= HS_XP_N && (d->ldy % 4) == 0, "taco_highway_stack_fwd: ldy %lld (>= 768, multiple of 4)", (long long)d->ldy);
+    TACO_CHECK(d->ldhw >= 128 && (d->ldhw % 4) == 0 && d->ldxp >= 128 && (d->ldxp % 4) == 0,
+               "taco_highway_stack_fwd: ldhw / ldxp must be >= 128 and multiples of 4");
+    TACO_CHECK(!d->Wd_p || (d->ldwd >= Cpad && (d->ldwd % 4) == 0), "taco_highway_stack_fwd: ldwd %lld (>= round_up(C,32), multiple of 4)",
+               (long long)d->ldwd);
+    return 0;
+}
+
+// xp column splits per tile: the most (of 1, 2, 3, 6) that keep every CTA on its own SM
+static int taco_highway_stack_split(int M) {
+    const int tiles = (M + HS_BM - 1) / HS_BM;
+    for (int s : {6, 3, 2})
+        if (tiles * s <= TACO_SMS) return s;
+    return 1;
+}
+
+int taco_highway_stack(const taco_highway_stack_desc* d, cudaStream_t st) {
+    if (int rc = taco_highway_stack_check(d)) return rc;
+    if (d->M == 0) return 0;
+    EncodeTiledFn enc = get_encode_fn();
+    TACO_CHECK(enc != nullptr, "cuTensorMapEncodeTiled driver entry point not available");
+    const bool dense = d->C != 128;
+    const int split = taco_highway_stack_split(d->M);
+    HsMaps maps;
+    HsArgs a;
+    a.M = d->M;
+    a.dense = dense ? 1 : 0;
+    a.nlayers = a.dense + d->L + 1;
+    a.kin = (d->C + 31) / 32;
+    a.xp_chunks = HS_XP_N / 128 / split;
+    if (int rc = encode_2d(enc, &maps.x, d->X, d->C, d->M, d->ldx, "X")) return rc;
+    int l = 0;
+    if (dense) {
+        if (int rc = encode_2d(enc, &maps.w[l], d->Wd_p, d->ldwd, 2 * 128, d->ldwd, "Wd")) return rc;
+        a.lo_row0[l] = 128; a.bias[l] = d->bd; ++l;
+    }
+    for (int h = 0; h < d->L; ++h, ++l) {
+        if (int rc = encode_2d(enc, &maps.w[l], d->hw_p[h], d->ldhw, 2 * 256, d->ldhw, "highway")) return rc;
+        a.lo_row0[l] = 256; a.bias[l] = d->hw_b[h];
+    }
+    if (int rc = encode_2d(enc, &maps.w[l], d->xp_p, d->ldxp, 2 * HS_XP_N, d->ldxp, "xp")) return rc;
+    a.lo_row0[l] = HS_XP_N; a.bias[l] = d->xp_b;
+    a.total_items = (dense ? a.kin : 0) + d->L * 2 * 4 + a.xp_chunks * 4;    // (without the dense, kin = 4)
+    a.Y = d->Y; a.ldy = d->ldy;
+    static bool configured = false;
+    if (!configured) {
+        TACO_CUDA(cudaFuncSetAttribute(highway_stack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HS_SMEM));
+        configured = true;
+    }
+    dim3 grid((unsigned)((d->M + HS_BM - 1) / HS_BM), (unsigned)split);
+    highway_stack_kernel<<<grid, HS_THREADS, HS_SMEM, st>>>(maps, a);
+    TACO_LAUNCH_CHECK();
+    return 0;
 }

@@ -284,15 +284,8 @@ def conv1d_banks(inputs, K=16, cout=128, scope=None):
 # ----------------------------------------------------------------------------------------------
 # highway (models/ops.py:27-46)
 # ----------------------------------------------------------------------------------------------
-def highway(inputs, units=128, scope=None):
-    sc = scope or current_scope()
-    rt = runtime(sc.store)
-    B, T, Cin = inputs.shape
-    if Cin != units:                                            # ops.py:29-30
-        Wd, bd = sc.p("Wd"), sc.p("bd")
-        inputs = linear(rt, inputs, Wd, packed_weight(rt, sc.name("Wd"), Wd, 1, Cin, units), units, bias=bd,
-                        tag=sc.name("d"))
-
+def _highway_weights(rt, sc, units):
+    """[WH | WT] [units, 2 units], [bH | bT] and the packed operand of one highway layer"""
     def build_w(old):
         w = torch.cat([sc.p("WH"), sc.p("WT")], dim=1)
         if old is not None:
@@ -306,7 +299,18 @@ def highway(inputs, units=128, scope=None):
         return b.contiguous()
     Whw = rt.get(("hw_w", sc.prefix), build_w)
     bhw = rt.get(("hw_b", sc.prefix), build_b)
-    Wp = packed_weight(rt, sc.name("hw"), Whw, 1, units, 2 * units)
+    return Whw, bhw, packed_weight(rt, sc.name("hw"), Whw, 1, units, 2 * units)
+
+
+def highway(inputs, units=128, scope=None):
+    sc = scope or current_scope()
+    rt = runtime(sc.store)
+    B, T, Cin = inputs.shape
+    if Cin != units:                                            # ops.py:29-30
+        Wd, bd = sc.p("Wd"), sc.p("bd")
+        inputs = linear(rt, inputs, Wd, packed_weight(rt, sc.name("Wd"), Wd, 1, Cin, units), units, bias=bd,
+                        tag=sc.name("d"))
+    Whw, bhw, Wp = _highway_weights(rt, sc, units)
     if _save is not None:                                       # train: keep [h_pre | t_pre] for the backward
         from .. import kernels as K
         Pm = linear(rt, inputs, Whw, Wp, 2 * units, bias=bhw, tag=sc.name("P"))
@@ -320,16 +324,44 @@ def highway(inputs, units=128, scope=None):
 highwaynet = highway
 
 
+def highway_stack(inputs, num_layers=4, scope=None):
+    """Inference: the width-fixing dense (inputs not 128 wide, ops.py:29-30), `num_layers` highway layers (scopes
+    highway0, highway1, ...) and the bi-GRU input products of the same scope as ONE kernel (taco_highway_stack_fwd,
+    fp32x3 only): the activations between the layers never leave the SM.  Returns xp [B,T,768], bit-identical to
+    highway() x num_layers followed by the products bidirectional_gru() computes itself."""
+    sc = scope or current_scope()
+    rt = runtime(sc.store)
+    assert rt.impl == L.IMPL_TC3, "the fused highway stack is implemented for precision 'fp32x3'"
+    assert 1 <= num_layers <= L.HIGHWAY_STACK_MAX
+    assert inputs.dim() == 3 and inputs.stride(2) == 1
+    B, T, Cin = inputs.shape
+    assert inputs.stride(0) == T * inputs.stride(1)
+    d = L.HighwayStackDesc()
+    d.X = inputs.data_ptr(); d.ldx = inputs.stride(1); d.M = B * T; d.C = Cin
+    if Cin != 128:
+        dsc = sc.sub("highway0")
+        Wd = dsc.p("Wd")
+        Wdp = packed_weight(rt, dsc.name("Wd"), Wd, 1, Cin, 128)
+        d.Wd_p = Wdp.data_ptr(); d.ldwd = Wdp.stride(0); d.bd = dsc.p("bd").data_ptr()
+    d.L = num_layers
+    for l in range(num_layers):
+        _, bhw, Wp = _highway_weights(rt, sc.sub(f"highway{l}"), 128)
+        d.hw_p[l] = Wp.data_ptr(); d.hw_b[l] = bhw.data_ptr(); d.ldhw = Wp.stride(0)
+    _, bx, Wxp = _gru_input_weights(rt, sc)
+    d.xp_p = Wxp.data_ptr(); d.ldxp = Wxp.stride(0); d.xp_b = bx.data_ptr()
+    xp = rt.buf(sc.name("xp"), (B, T, 768))
+    d.Y = xp.data_ptr(); d.ldy = xp.stride(1)
+    d.impl = rt.impl
+    L.check(L.lib().taco_highway_stack_fwd(C.byref(d), L.current_stream()), "taco_highway_stack_fwd")
+    return xp
+
+
 # ----------------------------------------------------------------------------------------------
 # bidirectional GRU (models/ops.py:118-128)
 # ----------------------------------------------------------------------------------------------
-def bidirectional_gru(inputs, gru_units=128, scope=None, h0=None):
-    """h0: None (zero state) or the [B,128] initial state of both directions (initial_state_fw = initial_state_bw,
-    models/ops.py:111-126)"""
-    sc = scope or current_scope()
-    rt = runtime(sc.store)
-    assert gru_units == 128 and inputs.shape[-1] == 128, "the persistent GRU kernel is specialised for 128 units"
-    B, T, Cin = inputs.shape
+def _gru_input_weights(rt, sc, Cin=128):
+    """Input-side operand of both GRU directions, [Wg_fw | Wc_fw | Wg_bw | Wc_bw][:Cin] [Cin, 768], its bias and its
+    packed form (the products xp that taco_bigru_fwd reads)"""
     fw, bw = sc.sub("gru_fw"), sc.sub("gru_bw")
 
     def build_w(old):
@@ -345,7 +377,25 @@ def bidirectional_gru(inputs, gru_units=128, scope=None, h0=None):
         return b.contiguous()
     Wx = rt.get(("gru_wx", sc.prefix), build_w)                  # [128, 768]
     bx = rt.get(("gru_bx", sc.prefix), build_b)
-    xp = linear(rt, inputs, Wx, packed_weight(rt, sc.name("gru_wx"), Wx, 1, Cin, 768), 768, bias=bx, tag=sc.name("xp"))
+    return Wx, bx, packed_weight(rt, sc.name("gru_wx"), Wx, 1, Cin, 768)
+
+
+def bidirectional_gru(inputs, gru_units=128, scope=None, h0=None, xp=None):
+    """h0: None (zero state) or the [B,128] initial state of both directions (initial_state_fw = initial_state_bw,
+    models/ops.py:111-126).  xp: the input products [B,T,768] when the caller has computed them (CBHG's fused highway
+    stack); `inputs` is then not read."""
+    sc = scope or current_scope()
+    rt = runtime(sc.store)
+    assert gru_units == 128, "the persistent GRU kernel is specialised for 128 units"
+    fw, bw = sc.sub("gru_fw"), sc.sub("gru_bw")
+    if xp is None:
+        assert inputs.shape[-1] == 128, "the persistent GRU kernel is specialised for 128 units"
+        B, T, Cin = inputs.shape
+        Wx, bx, Wxp = _gru_input_weights(rt, sc, Cin)
+        xp = linear(rt, inputs, Wx, Wxp, 768, bias=bx, tag=sc.name("xp"))
+    else:
+        assert xp.dim() == 3 and xp.shape[-1] == 768 and xp.is_contiguous()
+        B, T, Cin = xp.shape[0], xp.shape[1], 128
     out = rt.buf(sc.name("gru_out"), (B, T, 2 * gru_units))
     if h0 is None:
         L.check(L.lib().taco_bigru_fwd(L.ptr(xp), L.ptr(fw.p("Wg")[Cin:]), L.ptr(fw.p("Wc")[Cin:]), L.ptr(bw.p("Wg")[Cin:]),
@@ -436,6 +486,10 @@ def CBHG(inputs, speaker_embed=None, K=16, c=[128, 128, 128], gru_units=128, num
             Sv, us, h0 = _speaker_terms(sc, speaker_embed, num_highway_layers)
             if _save is not None:
                 _save[sc.name("spk_e")] = speaker_embed; _save[sc.name("spk_s")] = Sv; _save[sc.name("h0")] = h0
+        if (_save is None and trace is None and speaker_embed is None and rt.impl == L.IMPL_TC3 and gru_units == 128
+                and 1 <= num_highway_layers <= L.HIGHWAY_STACK_MAX):
+            # inference: highway layers + bi-GRU input products in one kernel, same bits as the layer-by-layer route below
+            return bidirectional_gru(None, gru_units, scope=sc, xp=highway_stack(h, num_highway_layers, scope=sc))
         for layer in range(num_highway_layers):
             hsc = sc.sub(f"highway{layer}")
             if speaker_embed is not None:                         # width-fixing dense of [h | tile(s_l)] (ops.py:29-30)
