@@ -4,7 +4,9 @@
 mkdir -p gpurun_out
 nvidia-smi > gpurun_out/nvsmi.txt 2>&1
 python -c "import torch; print(torch.cuda.get_device_name(0), torch.cuda.get_device_capability(0))" > gpurun_out/dev.txt 2>&1
-for f in ${TEST_FILES:-test_gpu_linear test_gpu_recurrent test_gpu_model test_gpu_train test_gpu_train_fullsize test_gpu_decoder_envelope test_gpu_z_audio test_gpu_z_data test_gpu_z_features test_gpu_z_resample test_gpu_z_summary test_gpu_z_trim test_gpu_z_longform test_gpu_zz_decoder_budget test_gpu_speaker_decoder test_gpu_guided_attention}; do
+# default: every GPU module, in sorted order (the z / zz prefixes put the slow or device-hungry ones last)
+DEFAULT_FILES=$(cd tests && ls test_gpu_*.py | LC_ALL=C sort | sed 's/\.py$//')
+for f in ${TEST_FILES:-$DEFAULT_FILES}; do
   echo "=== $f ===" 
   timeout 900 python -m pytest tests/$f.py -q -m gpu --tb=short -p no:cacheprovider ${PYTEST_ARGS} > gpurun_out/$f.log 2>&1
   echo "rc=$?" >> gpurun_out/$f.log

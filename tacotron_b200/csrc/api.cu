@@ -228,7 +228,7 @@ int taco_mask_rows(const float* X, const int32_t* length, float* Y, int B, int T
 }
 
 int taco_l1_loss_fwd(const float* a, const float* b, int64_t n, float* partial_ws, float* out, void* stream) {
-    TACO_CHECK(a && b && partial_ws && out && n >= 0, "taco_l1_loss_fwd: bad arguments");
+    TACO_CHECK(((a && b) || n == 0) && partial_ws && out && n >= 0, "taco_l1_loss_fwd: bad arguments");   // empty inputs may be NULL
     TACO_CHECK(taco_aligned16(a) && taco_aligned16(b), "taco_l1_loss_fwd: inputs must be 16-byte aligned");
     l1_stage1<<<L1_BLOCKS, 256, 0, (cudaStream_t)stream>>>(a, b, n, partial_ws);
     TACO_LAUNCH_CHECK();

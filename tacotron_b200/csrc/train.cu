@@ -690,8 +690,6 @@ int taco_guided_attention(float* dscore, float* loss, const float* align, const 
     return 0;
 }
 
-#ifndef TACO_HOST_EMU   /* the remaining entry points launch with <<<>>> directly (not part of the host emulation) */
-
 int taco_colsum(float* out, const float* A, int64_t lda, const float* Bm, int64_t ldb, const float* R, int64_t ldr, int M, int N,
                 void* stream) {
     TACO_CHECK(out && A && M >= 0 && N >= 0, "taco_colsum: bad arguments");
@@ -703,7 +701,7 @@ int taco_colsum(float* out, const float* A, int64_t lda, const float* Bm, int64_
     if (rowblocks < 1) rowblocks = 1;
     const int rpb = (M + rowblocks - 1) / rowblocks;
     rowblocks = (M + rpb - 1) / rpb;
-    colsum_kernel<<<dim3(colblocks, rowblocks), 256, 0, (cudaStream_t)stream>>>(out, A, lda, Bm, ldb, R, ldr, M, N, rpb);
+    TACO_LAUNCH(colsum_kernel, dim3(colblocks, rowblocks), 256, 0, (cudaStream_t)stream, out, A, lda, Bm, ldb, R, ldr, M, N, rpb);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -712,7 +710,7 @@ int taco_bias_act(float* C, int64_t ldc, int M, int N, const float* bias, int ac
     TACO_CHECK(C && M >= 0 && N >= 0, "taco_bias_act: bad arguments");
     const int64_t total = (int64_t)M * N;
     if (total == 0) return 0;
-    bias_act_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(C, ldc, M, N, bias, act);
+    TACO_LAUNCH(bias_act_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, C, ldc, M, N, bias, act);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -722,7 +720,7 @@ int taco_mul_shift(float* out, int64_t ldo, const float* X, int64_t ldx, const f
     TACO_CHECK(out && X && Hm, "taco_mul_shift: NULL");
     const int64_t total = (int64_t)M * N;
     if (total == 0) return 0;
-    mul_shift_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(out, ldo, X, ldx, Hm, ldh, M, N, shift, period);
+    TACO_LAUNCH(mul_shift_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, out, ldo, X, ldx, Hm, ldh, M, N, shift, period);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -734,7 +732,8 @@ int taco_epi_bwd(float* dZ, int64_t lddz, const float* dY, int64_t lddy, const f
     TACO_CHECK((scale == nullptr) == (shift == nullptr), "taco_epi_bwd: scale and shift go together");
     const int64_t total = (int64_t)M * N;
     if (total == 0) return 0;
-    epi_bwd_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(dZ, lddz, dY, lddy, Y, ldy, R, ldr, M, N, relu, scale, shift, gain);
+    TACO_LAUNCH(epi_bwd_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, dZ, lddz, dY, lddy, Y, ldy, R, ldr, M, N, relu,
+                scale, shift, gain);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -743,7 +742,7 @@ int taco_epi_fwd_keep(float* X, int64_t ldx, const uint8_t* keep, int M, int N, 
     TACO_CHECK(X && keep, "taco_epi_fwd_keep: NULL");
     const int64_t total = (int64_t)M * N;
     if (total == 0) return 0;
-    epi_fwd_keep_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(X, ldx, keep, M, N, gain);
+    TACO_LAUNCH(epi_fwd_keep_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, X, ldx, keep, M, N, gain);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -752,7 +751,7 @@ int taco_bn_param_grad(float* dgamma, float* dbeta, const float* S1, const float
                        void* stream) {
     TACO_CHECK(dgamma && dbeta && S1 && S2 && gamma && beta, "taco_bn_param_grad: NULL");
     if (N == 0) return 0;
-    bn_param_grad_kernel<<<(N + 255) / 256, 256, 0, (cudaStream_t)stream>>>(dgamma, dbeta, S1, S2, gamma, beta, N);
+    TACO_LAUNCH(bn_param_grad_kernel, (N + 255) / 256, 256, 0, (cudaStream_t)stream, dgamma, dbeta, S1, S2, gamma, beta, N);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -761,7 +760,7 @@ int taco_maxpool_bwd(float* dX, const float* dP, const float* X, int B, int T, i
     TACO_CHECK(dX && dP && X, "taco_maxpool_bwd: NULL");
     const int64_t total = (int64_t)B * T * C;
     if (total == 0) return 0;
-    maxpool_bwd_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(dX, dP, X, T, C, total);
+    TACO_LAUNCH(maxpool_bwd_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, dX, dP, X, T, C, total);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -770,7 +769,7 @@ int taco_highway_fwd(float* Y, int64_t ldy, const float* Pm, int64_t ldp, const 
     TACO_CHECK(Y && Pm && X, "taco_highway_fwd: NULL");
     const int64_t total = (int64_t)M * U;
     if (total == 0) return 0;
-    highway_fwd_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(Y, ldy, Pm, ldp, X, ldx, M, U);
+    TACO_LAUNCH(highway_fwd_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, Y, ldy, Pm, ldp, X, ldx, M, U);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -780,7 +779,8 @@ int taco_highway_bwd(float* dP, int64_t lddp, float* dXd, int64_t lddx, const fl
     TACO_CHECK(dP && dXd && dY && Pm && X, "taco_highway_bwd: NULL");
     const int64_t total = (int64_t)M * U;
     if (total == 0) return 0;
-    highway_bwd_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(dP, lddp, dXd, lddx, dY, lddy, Pm, ldp, X, ldx, M, U);
+    TACO_LAUNCH(highway_bwd_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, dP, lddp, dXd, lddx, dY, lddy, Pm, ldp, X,
+                ldx, M, U);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -788,7 +788,7 @@ int taco_highway_bwd(float* dP, int64_t lddp, float* dXd, int64_t lddx, const fl
 int taco_l1_bwd(float* dA, const float* A, const float* Bt, int64_t n, float beta, void* stream) {
     TACO_CHECK(dA && A && Bt && n >= 0, "taco_l1_bwd: bad arguments");
     if (n == 0) return 0;
-    l1_bwd_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(dA, A, Bt, n, beta);
+    TACO_LAUNCH(l1_bwd_kernel, grid_for(n, 256), 256, 0, (cudaStream_t)stream, dA, A, Bt, n, beta);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -796,7 +796,7 @@ int taco_l1_bwd(float* dA, const float* A, const float* Bt, int64_t n, float bet
 int taco_l1_bwd_ld(float* dA, int64_t ldd, const float* A, const float* Bt, int64_t rows, int64_t cols, float beta, void* stream) {
     TACO_CHECK(dA && A && Bt && rows >= 0 && cols >= 0 && ldd >= cols, "taco_l1_bwd_ld: bad arguments");
     if (rows * cols == 0) return 0;
-    l1_bwd_ld_kernel<<<grid_for(rows * cols, 256), 256, 0, (cudaStream_t)stream>>>(dA, ldd, A, Bt, rows, cols, beta);
+    TACO_LAUNCH(l1_bwd_ld_kernel, grid_for(rows * cols, 256), 256, 0, (cudaStream_t)stream, dA, ldd, A, Bt, rows, cols, beta);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -805,7 +805,7 @@ int taco_scatter_add_rows(float* dTable, const int32_t* ids, const float* dRows,
     TACO_CHECK(dTable && ids && dRows && vocab > 0, "taco_scatter_add_rows: bad arguments");
     const int64_t total = (int64_t)rows * width;
     if (total == 0) return 0;
-    scatter_add_rows_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(dTable, ids, dRows, rows, width, vocab);
+    TACO_LAUNCH(scatter_add_rows_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, dTable, ids, dRows, rows, width, vocab);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -816,7 +816,7 @@ int taco_dec_inputs(float* Xin, uint8_t* sel, const float* mel, const float* y, 
     TACO_CHECK(!sched || (y && sample_mask), "taco_dec_inputs: scheduled sampling needs y and sample_mask");
     const int64_t total = (int64_t)T * B * 80;
     if (total == 0) return 0;
-    dec_inputs_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(Xin, sel, mel, y, sample_mask, B, T, r, 80, sched);
+    TACO_LAUNCH(dec_inputs_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, Xin, sel, mel, y, sample_mask, B, T, r, 80, sched);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -825,16 +825,16 @@ int taco_attn_bwd_post(float* dkeys, float* dv, const float* DSCORE, const float
                        int Tx, void* stream) {
     TACO_CHECK(dkeys && dv && DSCORE && keys && PQ && v, "taco_attn_bwd_post: NULL");
     if (B * Tx == 0) return 0;
-    attn_bwd_post_kernel<<<B * Tx, 256, 0, (cudaStream_t)stream>>>(dkeys, dv, DSCORE, keys, PQ, v, B, T, Tx);
+    TACO_LAUNCH(attn_bwd_post_kernel, B * Tx, 256, 0, (cudaStream_t)stream, dkeys, dv, DSCORE, keys, PQ, v, B, T, Tx);
     TACO_LAUNCH_CHECK();
     return 0;
 }
 
 int taco_sumsq(const float* x, int64_t n, float* partial_ws, float* out, void* stream) {
-    TACO_CHECK(x && partial_ws && out && n >= 0, "taco_sumsq: bad arguments");
-    sumsq_stage1<<<SS_BLOCKS, 256, 0, (cudaStream_t)stream>>>(x, n, partial_ws);
+    TACO_CHECK((x || n == 0) && partial_ws && out && n >= 0, "taco_sumsq: bad arguments");   // an empty x may be NULL
+    TACO_LAUNCH(sumsq_stage1, SS_BLOCKS, 256, 0, (cudaStream_t)stream, x, n, partial_ws);
     TACO_LAUNCH_CHECK();
-    sumsq_stage2<<<1, 1024, 0, (cudaStream_t)stream>>>(partial_ws, SS_BLOCKS, out);
+    TACO_LAUNCH(sumsq_stage2, 1, 1024, 0, (cudaStream_t)stream, partial_ws, SS_BLOCKS, out);
     TACO_LAUNCH_CHECK();
     return 0;
 }
@@ -843,11 +843,9 @@ int taco_adam_step(float* p, const float* g, float* m, float* v, int64_t n, floa
                    const float* sumsq, void* stream) {
     TACO_CHECK(p && g && m && v && sumsq && n >= 0, "taco_adam_step: bad arguments");
     if (n == 0) return 0;
-    adam_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, lr_t, b1, b2, eps, clip, sumsq);
+    TACO_LAUNCH(adam_kernel, grid_for(n, 256), 256, 0, (cudaStream_t)stream, p, g, m, v, n, lr_t, b1, b2, eps, clip, sumsq);
     TACO_LAUNCH_CHECK();
     return 0;
 }
-
-#endif  /* !TACO_HOST_EMU */
 
 }  // extern "C"

@@ -65,6 +65,15 @@ inline float __shfl_xor_sync(unsigned, float v, int lane_mask) {
     c.warp_bar->arrive_and_wait();
     return r;
 }
+inline double __shfl_xor_sync(unsigned, double v, int lane_mask) {      // two exchange words per lane
+    auto& c = emu::ctx;
+    memcpy(c.warp_xf + 2 * c.lane, &v, sizeof v);
+    c.warp_bar->arrive_and_wait();
+    double r;
+    memcpy(&r, c.warp_xf + 2 * (c.lane ^ lane_mask), sizeof r);
+    c.warp_bar->arrive_and_wait();
+    return r;
+}
 
 // mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 by its PTX definition:
 //   A (16x8, row): a0 (g, tg) a1 (g+8, tg) a2 (g, tg+4) a3 (g+8, tg+4);  B (8x8, col): b0 (k=tg, n=g) b1 (k=tg+4, n=g)

@@ -1,6 +1,7 @@
 // emu_lib.cpp -- TEST INFRASTRUCTURE ONLY.  Builds libtaco_emu.so: the product's own kernel sources (audio.cu, data.cu,
-// the two GEMM kernels of train.cu) compiled with g++ over tests/cuda_emu/emu.h, exporting the SAME C-ABI entry points
-// (taco_gemm, taco_set_gemm_impl, taco_gl_*, taco_normalize_f16) so that tests/test_cuda_emu.py can drive them through
+// every kernel of train.cu) compiled with g++ over tests/cuda_emu/emu.h, exporting the SAME C-ABI entry points
+// (taco_gemm, taco_set_gemm_impl, taco_bias_act, ..., taco_gl_*, taco_normalize_f16) so that tests/test_cuda_emu.py and
+// tests/test_train_envelope_host.py can drive them through
 // ctypes with host pointers and compare with the torch-CPU mirrors -- no GPU involved.
 #include "emu.h"
 

@@ -37,7 +37,7 @@ def _shift_rows(A, sh, period):
     R = A.shape[0]
     period = period or R
     out = torch.zeros_like(A)
-    idx = torch.arange(R)
+    idx = torch.arange(R, device=A.device)
     src = idx + sh
     ok = (src >= 0) & (src < R) & (torch.div(idx, period, rounding_mode="floor") == torch.div(src.clamp(0, R - 1), period, rounding_mode="floor"))
     out[idx[ok]] = A[src[ok]]
@@ -62,7 +62,7 @@ def gemm(C, A, B, *, ta=False, tb=False, beta=0.0, shift=0, period=0, taps=1, ds
         Az = _offset_view(A, z * a_bstride)
         Bz = _offset_view(B, z * b_bstride)
         sh0 = shift + z * bshift
-        acc = torch.zeros(M, N, dtype=C.dtype)
+        acc = torch.zeros(M, N, dtype=C.dtype, device=C.device)
         if ta:
             assert taps == 1
             Ash = _shift_rows(Az, sh0, period)                 # [K, M]
