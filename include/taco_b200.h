@@ -200,7 +200,8 @@ size_t taco_decoder_workspace_bytes(int B, int Tx, int T, int r);
 int taco_decoder_pack(const taco_decoder_weights* w, int r, float* packed, void* stream);
 
 typedef struct taco_decoder_args {
-    const taco_decoder_weights* weights; /* HOST pointer; biases and attention_v are read from here */
+    const taco_decoder_weights* weights; /* HOST pointer; biases and attention_v are read from here (in_b and
+                                            gru_bg[0] were folded in by taco_decoder_pack)              */
     const float*   packed;       /* from taco_decoder_pack                                    */
     const float*   keys;         /* [B][Tx][256]  values . W_mem                              */
     const float*   values;       /* [B][Tx][256]  length-masked memory                        */

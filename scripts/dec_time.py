@@ -29,9 +29,9 @@ print("precision", args.precision, "decoder ms", statistics.median(dec), "step p
 if os.environ.get("TACO_TRACE"):
     import numpy as np
     ws = m.runtime.dec_ws.view(torch.int64).cpu().numpy()
-    total = (11 * 32 + 48) * 4 * 64             # exchange buffers [4 row groups][nkt][8][8] words (decoder.cu build_ws_layout)
+    total = (10 * 32 + 48) * 4 * 64             # exchange buffers [4 row groups][nkt][8][8] words (decoder.cu build_ws_layout)
     total += 32 * 2 * 4 * (2 + 256)             # + attention exchange [32 utterances][2][4] x (2 statistics + 256 context words)
-    names = ["IN", "G1", "C1", "G2", "C2", "G3", "C3", "OQP", "A|P2"]
+    names = ["G1", "C1", "G2", "C2", "G3", "C3", "OQP", "A|P2"]
     n = 1 + len(names) * T
     tr = ws[total: total + n]
     d = np.diff(tr)                              # d[i] = time of entry i+1 - entry i; entry 0 = prologue
@@ -39,7 +39,7 @@ if os.environ.get("TACO_TRACE"):
     med = np.median(d, axis=0)
     print("per-slot median ns (CTA 0):", {n_: int(v) for n_, v in zip(names, med)}, "sum", int(med.sum()))
     ck = ws[total + 16 * T + 16: total + 16 * T + 16 + 4 * 20 * 8].reshape(4, 20, 8)
-    inames = ["IN", "G1", "C1", "G2", "C2", "G3", "C3", "OQP", "AP2"]
+    inames = ["G1", "C1", "G2", "C2", "G3", "C3", "OQP", "AP2"]
     print("stage: start->on-chain loads issued | (off-chain half) ->on-chain weights | ->mma done | (finish) ->partials | ->sync | ->epilogue"
           "   [cycles, CTA0 thread0, median of steps 10..12]")
     for i, nm in enumerate(inames):
@@ -50,7 +50,7 @@ if os.environ.get("TACO_TRACE"):
         nxt = [ck[st, i + 1, 3] if i + 1 < len(inames) else ck[st + 1, 0, 3] for st in range(3)]
         total = int(statistics.median([int(nxt[st] - ck[st, i, 3]) for st in range(3)]))
         print(f"  {nm:8s} {f(0,3):6d} {f(1,0):6d} {f(2,1):6d} | {f(4,2):6d} {f(5,4):6d} {f(6,5):6d} | total {total:6d}")
-    c = ck[:3, 8]     # A|P2 stage records: attention on warp 0 / thread 0
+    c = ck[:3, 7]     # A|P2 stage records: attention on warp 0 / thread 0
     if c[1, 3]:
         print("attention (cycles from slot start): q arrived+exp %d | bar1 %d | scores %d | bar2 %d | stats+bar3 %d | ctx partial+push %d | merged ctx stored %d"
               % tuple(int(statistics.median([int(c[st, i] - c[st, 3]) for st in range(3)])) for i in (0, 1, 2, 4, 5, 6, 7)))

@@ -1,4 +1,4 @@
-// decoder.cu -- the whole autoregressive attention decoder as ONE persistent dataflow kernel (design v4).
+// decoder.cu -- the whole autoregressive attention decoder as ONE persistent dataflow kernel (design v5).
 //
 // Reference: models/tacotron.py:46-105 (create_decoder) + :136-138 (dynamic_decode) over the
 // TF-1.2 contrib.seq2seq / contrib.rnn classes (SURVEY.md A.5-A.10).  Per decoder step t:
@@ -25,6 +25,10 @@
 //     the attention on warps 0-3 and the second pre-net layer on warps 4-7 concurrently; IN takes y(t-1) through
 //     s(t-1).(W_out W_a[:80r] W_in[128:]) so y never travels.  Teacher-forced rows take p1 from a separate
 //     off-chain stage PM (mel . W1), selected per row by the consumer.
+//   * v5: 8 dependent slots, G1 C1 G2 C2 G3 C3 OQP A|P2.  IN only produced z(t), which the chain needs through z . Wg1_x,
+//     z . Wc1_x and the residual s = z + h3 alone: G1 multiplies [ctx(t-1) | p2(t)] and s(t-1) by the pack-time products
+//     of IN's weights with Wg1_x and [Wc1_x | I] (fused_tail), into a gate tile and a [C1 x-half | z] tile; the second
+//     tile stays in the CTA (cx_loc, z_loc), so C1 has no off-chain half and no stage publishes z.
 //   * every K=512 contraction is split into the half that is on the dependent chain (x of the gates, r*h of the
 //     candidate, ctx/p2 of the input projection) and the half whose operand has been known for a while (h(t-1), x,
 //     s(t-1)).  The known half is multiplied in the shadow of the previous slot's L2 hop into the SAME accumulator
@@ -34,7 +38,7 @@
 //     which stays in the 50 MB L2.  They are loaded one stage early, together with the off-chain operand words, so
 //     they travel while the previous stage's epilogue runs (loaded at the start of their own stage, their L2 latency
 //     made the off-chain half ~400 cycles longer than the on-chain operand's hop on an H100, so it sat on the chain).
-//     Only IN, the first stage of a step, loads them in place.
+//     Only the first stage of a step loads them in place.
 //   * MMA orientation swapped: M = 16 weight columns of the CTA's slice, N = the 8 utterance rows of the CTA's row
 //     group, so the 16-column gate stage has no zero-padded rows (half the MMAs of v3).
 //   * attention: the four CTAs that share an utterance (blockIdx / 4) each score a quarter of the memory; partial softmax
@@ -72,25 +76,27 @@ constexpr int KV_LD = 260;     // padded row stride of e^{2 keys} in smem
 constexpr int PPITCH = 132;    // floats between the partial tiles of consecutive warps (128 + 4: cross-warp sums hit different banks)
 
 // ---- weight segments (one K slab of one stage, per CTA column slice) ---------------------------------------------
+//      The first GRU's gate and candidate products take the input projection z = [ctx | p2] . W_cpF + s(t-1) . W_sF +
+//      b_inF folded in (see fused_tail): G1_* = the gates, Z1_* = [candidate x-half | z] of the same 8 units.
 enum SegId {
-    SG_IN_S = 0, SG_IN_CP,
-    SG_G_H0, SG_G_H1, SG_G_H2, SG_G_X0, SG_G_X1, SG_G_X2,
-    SG_C_X0, SG_C_X1, SG_C_X2, SG_C_RH0, SG_C_RH1, SG_C_RH2,
+    SG_G1_CP = 0, SG_Z1_CP, SG_G1_S, SG_Z1_S,
+    SG_G_H0, SG_G_H1, SG_G_H2, SG_G_X1, SG_G_X2,
+    SG_C_X1, SG_C_X2, SG_C_RH0, SG_C_RH1, SG_C_RH2,
     SG_Y, SG_QP, SG_PM, SG_P2, NSEG
 };
 // ---- exchange buffers: [4 row groups][nkt k-tiles][8 rows][8 words] of 64-bit {value, tag} words.  One k-tile of one
 //      row group (512 B) is written by ONE producer CTA and read by one warp-wide 16-byte load: fully coalesced.
-//      B_CP holds ctx (k-tiles 0..31) and p2 (k-tiles 32..47): the on-chain operand of the input projection.
-enum BufId { B_S = 0, B_CP, B_Z, B_H0, B_H1, B_H2, B_RH0, B_RH1, B_RH2, B_Q, B_P1Y, B_P1M, NBUF };
+//      B_CP holds ctx (k-tiles 0..31) and p2 (k-tiles 32..47): the on-chain operand of the first GRU stage.
+enum BufId { B_S = 0, B_CP, B_H0, B_H1, B_H2, B_RH0, B_RH1, B_RH2, B_Q, B_P1Y, B_P1M, NBUF };
 __host__ __device__ inline int buf_nkt(int b) { return b == B_CP ? 48 : 32; }
 // ---- stages (what "finish" does) --------------------------------------------------------------------------------
-enum StageId { ST_IN = 0, ST_G0, ST_G1, ST_G2, ST_C0, ST_C1, ST_C2, ST_PM, ST_OQP, ST_AP2, ST_NONE };
-// bias rows in smem ([row][16])
-enum BiasRow { BR_IN = 0, BR_INX, BR_G0, BR_G1, BR_G2, BR_C0, BR_C1, BR_C2, BR_Y, BR_QP, BR_PM, BR_P2, NBR };
+enum StageId { ST_G0 = 0, ST_G1, ST_G2, ST_C0, ST_C1, ST_C2, ST_PM, ST_OQP, ST_AP2, ST_NONE };
+// bias rows in smem ([row][16]); BR_G0 / BR_Z1 hold the step t > 0 biases of the first stage, BR_G0T / BR_Z1T those of t = 0
+enum BiasRow { BR_G0 = 0, BR_G1, BR_G2, BR_G0T, BR_Z1, BR_Z1T, BR_C0, BR_C1, BR_C2, BR_Y, BR_QP, BR_PM, BR_P2, NBR };
 // item kinds: fragment width / tiles / k-tile slots per warp
-enum ItemKind { IK_F2 = 0, IK_F4, IK_F4X2, IK_F2CP, IK_PM, IK_AP2 };   // 8 / 16 / 2x16 columns x 2 k-tile slots; [ctx|p2]: 3 slots
+enum ItemKind { IK_F2 = 0, IK_F4, IK_F4X2, IK_G1, IK_PM, IK_AP2 };   // 8 / 16 / 2x16 columns x 2 k-tile slots; G1: 2x16 x 3 slots
 // output slots of the per-CTA output-offset table
-enum OutId { O_Z = 0, O_RH0, O_RH1, O_RH2, O_H0, O_H1, O_H2, O_S, O_Q, O_P1Y, O_P1M, O_P2, NOUT };
+enum OutId { O_RH0 = 0, O_RH1, O_RH2, O_H0, O_H1, O_H2, O_S, O_Q, O_P1Y, O_P1M, O_P2, NOUT };
 
 struct SegDesc {
     int K;             // contraction length (multiple of 8)
@@ -121,17 +127,19 @@ struct DecParams {
     int64_t att_off;             // word offset of the attention exchange region
     int64_t trace_off;
     taco_decoder_args a;
-    const float *in_b, *gru_bg[3], *gru_bc[3], *out_b, *pre_b1, *pre_b2, *att_v;
-    const float *b_qF, *b_p1F, *b_inS;     // fused biases (packed tail)
-    const float *init_z, *init_g;          // step-0 terms of a non-zero initial state (workspace tail), or NULL:
-                                           //   att0 . W_in[128:] [32][256],  h0_i . Wg_i[256:] [3][32][512]
+    const float *gru_bg[3], *gru_bc[3], *out_b, *pre_b1, *pre_b2, *att_v;
+    const float *b_qF, *b_p1F;             // fused biases (packed tail)
+    const float *b_g1F, *b_g1F0, *b_z1F, *b_z1F0;
+    const float *init_z, *init_zg, *init_g;   // step-0 terms of a non-zero initial state (workspace tail), or NULL, with
+                                              // iz = att0 . W_in[128:]:  [iz . Wc1_x | iz] [32][512],  iz . Wg1_x [32][512],
+                                              // h0_i . Wg_i[256:] [3][32][512]
     int OUT, NCY, Tq;
     int smem_kv_off, smem_res_off, smem_total_floats;
 };
 
 // global column computed by weight-column m (0..15) of slice cs for a segment (-1 = padding)
 __host__ __device__ inline int seg_col(int sg, int cs, int m, int NCY, int OUT) {
-    if (sg >= SG_G_H0 && sg <= SG_G_X2) return (m < 8) ? (8 * cs + m) : (U + 8 * cs + (m - 8));     // r | u of units 8cs..8cs+7
+    if (sg <= SG_G_X2) return (m < 8) ? (8 * cs + m) : (U + 8 * cs + (m - 8));     // r | u (Z1: candidate | z) of units 8cs..8cs+7
     if (sg == SG_QP) return (m < 8) ? (8 * cs + m) : (AU + 8 * cs + (m - 8));                       // q | p1' (source = [W_qF | W_p1F])
     if (sg == SG_Y) { const int c = cs * NCY + m; return (m < NCY && c < OUT) ? c : -1; }
     if (sg == SG_P2) return (m < 4) ? (4 * cs + m) : -1;
@@ -296,26 +304,30 @@ __device__ __forceinline__ void consume(float (&acc)[2][3][4], ulonglong2 (&v)[4
     multiply<FL, MT, NS_, TR>(acc, v, w, p0, nkt, widx, nw, s0, tag, ck);
 }
 
-struct ItemRec { uint32_t flags, pre_base; int pre_tagd; uint32_t pre_w; uint32_t on_base; int on_tagd; uint32_t on_w1, on_w2; int on_nkt, pad0, pad1, pad2; };   // 48 bytes, in smem
+struct ItemRec { uint32_t flags, pre_base; int pre_tagd; uint32_t pre_w; uint32_t on_base; int on_tagd; uint32_t on_w1, on_w2; int on_nkt;
+                 uint32_t s_base, s_w1, s_w2; };   // 48 bytes, in smem
 // flags: kind | stage << 8 | has_pre << 16 | pre_skip0 << 17 | on_s0 << 20
+// s_*: the second off-chain operand of the G1 item, s(t-1), and its two weight tiles (SG_G1_S, SG_Z1_S)
 
 template <bool TR>     // TR: per-stage clock64 trace of CTA 0 (scripts/dec_time.py); the production instantiation has none of it
 __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant__ DecParams P) {
     extern __shared__ __align__(16) float smem[];
-    // smem map (floats): [0,16) reserved | part 6400 | part2 512 | loc 384 | bias 256 | att 704 | reserved 1088 | itab 256 | kv | weights
-    float* part_s = smem + 16;                                    // [3 buffers][16 warps][PPITCH]: two alternate, the third is OQP's 2nd tile
+    // smem map (floats): [0,16) reserved | part 6400 | part2 512 | loc 384 | bias 256 | att 704 | itab 256 | kv | weights
+    float* part_s = smem + 16;                                    // [3 buffers][16 warps][PPITCH]: two alternate, the third is the
+                                                                  // 2nd tile of OQP and G1
     float* part2_s = part_s + 6400;                               // [8 warps][64]   (P2, warps 8-15)
-    float* loc_s = part2_s + 512;                                 // h_loc[3][64] | u_loc[64] | z_loc[64]
+    float* loc_s = part2_s + 512;                                 // h_loc[3][64] | u_loc[64] | z_loc[64] | cx_loc[64]
     float* bias_s = loc_s + 384;                                  // [NBR][16]
     float* att_s = bias_s + 256;                                  // eq[256] | v[256] | e[64] | p[64] | misc[64]
-    ItemRec* itab = reinterpret_cast<ItemRec*>(att_s + 704 + 1024 + 64);   // [MAX_ITEMS] resolved stage records (20 x 12 words)
+    ItemRec* itab = reinterpret_cast<ItemRec*>(att_s + 704);                 // [MAX_ITEMS] resolved stage records (20 x 12 words)
     uint32_t* otab = reinterpret_cast<uint32_t*>(itab + MAX_ITEMS);          // [NOUT] output word offsets of this CTA
     float* ek_s = smem + P.smem_kv_off;
     float* vals_s = ek_s + P.Tq * KV_LD;
     float* res_s = smem + P.smem_res_off;
     float* h_loc = loc_s;             // [3][8 cols][8 rows]
     float* u_loc = loc_s + 192;
-    float* z_loc = loc_s + 256;
+    float* z_loc = loc_s + 256;       // z(t): the residual term of s = z + h3
+    float* cx_loc = loc_s + 320;      // z(t) . Wc1_x + its bias terms: the x-half of the first candidate, formed by G1
     float* eq_s = att_s;
     float* v_s = att_s + 256;
     float* e_s = att_s + 512;
@@ -351,10 +363,12 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
         float bv = 0.f;
         int col; const float* bp = nullptr;
         switch (br) {
-            case BR_IN:  col = seg_col(SG_IN_CP, cs, m, NCY, OUT); bp = P.in_b; break;
-            case BR_INX: col = seg_col(SG_IN_CP, cs, m, NCY, OUT); bp = P.b_inS; break;
-            case BR_G0: case BR_G1: case BR_G2: col = seg_col(SG_G_X0, cs, m, NCY, OUT); bp = P.gru_bg[br - BR_G0]; break;
-            case BR_C0: case BR_C1: case BR_C2: col = seg_col(SG_C_X0, cs, m, NCY, OUT); bp = P.gru_bc[br - BR_C0]; break;
+            case BR_G0:  col = seg_col(SG_G1_CP, cs, m, NCY, OUT); bp = P.b_g1F; break;
+            case BR_G0T: col = seg_col(SG_G1_CP, cs, m, NCY, OUT); bp = P.b_g1F0; break;
+            case BR_Z1:  col = seg_col(SG_Z1_CP, cs, m, NCY, OUT); bp = P.b_z1F; break;
+            case BR_Z1T: col = seg_col(SG_Z1_CP, cs, m, NCY, OUT); bp = P.b_z1F0; break;
+            case BR_G1: case BR_G2: col = seg_col(SG_G_X1, cs, m, NCY, OUT); bp = P.gru_bg[br - BR_G0]; break;
+            case BR_C0: case BR_C1: case BR_C2: col = seg_col(SG_C_X1, cs, m, NCY, OUT); bp = P.gru_bc[br - BR_C0]; break;
             case BR_Y:   col = seg_col(SG_Y, cs, m, NCY, OUT); bp = P.out_b; break;
             case BR_QP:  col = (m < 8) ? 8 * cs + m : 8 * cs + (m - 8); bp = (m < 8) ? P.b_qF : P.b_p1F; break;
             case BR_PM:  col = seg_col(SG_PM, cs, m, NCY, OUT); bp = P.pre_b1; break;
@@ -380,10 +394,14 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             r.on_tagd = it.on_tagd; r.on_w1 = wword(it.on_seg); r.on_w2 = it.on_seg2 >= 0 ? wword(it.on_seg2) : 0u;
             r.on_nkt = P.seg[it.on_seg].K >> 3;
         }
+        if (it.kind == IK_G1) {
+            r.s_base = (uint32_t)(P.buf[B_S] + (int64_t)rg * buf_nkt(B_S) * 64);
+            r.s_w1 = wword(SG_G1_S); r.s_w2 = wword(SG_Z1_S);
+        }
         itab[tid] = r;
     }
     if (tid < NOUT) {
-        const int bmap[NOUT] = {B_Z, B_RH0, B_RH1, B_RH2, B_H0, B_H1, B_H2, B_S, B_Q, B_P1Y, B_P1M, B_CP};
+        const int bmap[NOUT] = {B_RH0, B_RH1, B_RH2, B_H0, B_H1, B_H2, B_S, B_Q, B_P1Y, B_P1M, B_CP};
         const int b = bmap[tid];
         uint32_t o = (uint32_t)(P.buf[b] + (int64_t)rg * buf_nkt(b) * 64);
         if (tid == O_P2) o += (uint32_t)((32 + (cs >> 1)) * 64 + 0);     // p2 columns 4cs..4cs+3 live in k-tile 32 + cs/2 of B_CP
@@ -683,39 +701,43 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
 
     auto finish = [&](int stage, int t) {
         float* part = part_s + par * (NWARP * PPITCH);
-        float* part_b = part_s + 2 * (NWARP * PPITCH);               // second tile of OQP (its previous readers are a full step behind)
+        float* part_b = part_s + 2 * (NWARP * PPITCH);               // second tile of OQP and G1
         par ^= 1;
         const bool full16 = (stage >= ST_G0 && stage <= ST_G2) || stage == ST_OQP;
-        store_partials(part, part_b, stage == ST_OQP ? 2 : 1, full16);
+        // part_b was last read by the OQP epilogue just before; the attention and pre-net warps in between do not wait
+        // for each other, so every warp must be past that epilogue before G1 overwrites it
+        if (stage == ST_G0) __syncthreads();
+        store_partials(part, part_b, (stage == ST_OQP || stage == ST_G0) ? 2 : 1, full16);
         if (TR && cktr) cktr[4] = clock64();
         __syncthreads();
         if (TR && cktr) cktr[5] = clock64();
         const uint32_t tag = (uint32_t)t + 1;
         switch (stage) {
-            case ST_IN:
-                if (tid < 64) {
-                    float zv = sum16(part, e_pidx) + bias_s[BR_IN * 16 + e_wc];
-                    if (t > 0) zv += bias_s[BR_INX * 16 + e_wc];
-                    else if (P.init_z && e_row < B) zv += P.init_z[e_row * U + 8 * cs + e_wc];      // att0 . W_in[128:]
-                    z_loc[e_loc] = zv;
-                    ll_store(ws + otab[O_Z] + e_word, zv, tag);
-                }
-                break;
             case ST_G0: case ST_G1: case ST_G2:
                 if (tid < 128) {
                     const int gi = stage - ST_G0;
-                    float gp = sum16(part, e_pidx) + bias_s[(BR_G0 + gi) * 16 + e_wc + 8 * e_hi];
-                    if (t == 0 && P.init_g && e_row < B)                                          // h0_i . Wg_i[256:]
-                        gp += P.init_g[((int64_t)gi * BPAD + e_row) * 2 * U + U * e_hi + 8 * cs + e_wc];
+                    const int br = (gi == 0 && t == 0) ? BR_G0T : BR_G0 + gi;
+                    float gp = sum16(part, e_pidx) + bias_s[br * 16 + e_wc + 8 * e_hi];
+                    if (t == 0 && e_row < B) {
+                        const int64_t ci = (int64_t)e_row * 2 * U + U * e_hi + 8 * cs + e_wc;
+                        if (P.init_g) gp += P.init_g[(int64_t)gi * BPAD * 2 * U + ci];             // h0_i . Wg_i[256:]
+                        if (gi == 0 && P.init_zg) gp += P.init_zg[ci];                         // att0 . W_in[128:] . Wg1_x
+                    }
                     const float gt = sigmoidf_acc(gp);
                     if (!e_hi) ll_store(ws + otab[O_RH0 + gi] + e_word, gt * h_loc[gi * 64 + e_loc], tag);   // r * h
                     else u_loc[e_loc] = gt;                                                                // u stays local
+                } else if (stage == ST_G0 && tid < 256) {                 // second tile: candidate x-half (e_hi = 0) | z (e_hi = 1)
+                    float zv = sum16(part_b, e_pidx) + bias_s[(t == 0 ? BR_Z1T : BR_Z1) * 16 + e_wc + 8 * e_hi];
+                    if (t == 0 && P.init_z && e_row < B) zv += P.init_z[(int64_t)e_row * 2 * U + U * e_hi + 8 * cs + e_wc];
+                    (e_hi ? z_loc : cx_loc)[e_loc] = zv;
                 }
                 break;
             case ST_C0: case ST_C1: case ST_C2:
                 if (tid < 64) {
                     const int gi = stage - ST_C0;
-                    const float cnd = tanhf_acc(sum16(part, e_pidx) + bias_s[(BR_C0 + gi) * 16 + e_wc]);
+                    float cp = sum16(part, e_pidx) + bias_s[(BR_C0 + gi) * 16 + e_wc];
+                    if (gi == 0) cp += cx_loc[e_loc];
+                    const float cnd = tanhf_acc(cp);
                     const float uu = u_loc[e_loc];
                     const float hn = uu * h_loc[gi * 64 + e_loc] + (1.0f - uu) * cnd;
                     h_loc[gi * 64 + e_loc] = hn;
@@ -769,7 +791,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     float wpre[8];                                      // and its weight fragments (FL = 4: 2 slots x 4 floats; FL = 2: the first 4)
     bool pref = false;                                  // vp[] / wpre[] already hold the loads of the current stage's off-chain half
     auto load_pre_weights = [&](int knd, uint32_t ww) {
-        if (knd == IK_F4) load_weights<4, 1, 2>(wpre, ww, 0u, warp * 2, res_s, packed, lane);
+        if (knd == IK_F4 || knd == IK_G1) load_weights<4, 1, 2>(wpre, ww, 0u, warp * 2, res_s, packed, lane);
         else              load_weights<2, 1, 2>(wpre, ww, 0u, warp * 2, res_s, packed, lane);
     };
     auto ld_rec = [&](int ii, uint4& r0, uint4& r1, uint32_t& nkt) {
@@ -802,28 +824,46 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             // ---- on-chain operand: loads in flight first, they travel while the off-chain half is multiplied ----
             const uint64_t* pon = ws + r1.x + warp * 64 + lane_w;
             const int s0 = (t == 0) ? (int)((r0.x >> 20) & 0xf) : 0;
-            if (kind == IK_F2CP) issue_loads<3>(v, pon, (int)on_nkt, warp, NWARP, s0);
-            else                 issue_loads<2>(v, pon, (int)on_nkt, warp, NWARP, 0);
+            if (kind == IK_G1) issue_loads<3>(v, pon, (int)on_nkt, warp, NWARP, s0);
+            else               issue_loads<2>(v, pon, (int)on_nkt, warp, NWARP, 0);
             if (TR && ck) ck[0] = clock64();
             const bool has_pre = ((r0.x >> 16) & 1) && !(t == 0 && ((r0.x >> 17) & 1));
             const uint64_t* ppre = ws + r0.y + warp * 64 + lane_w;
             const uint32_t ptag = (uint32_t)(t + (int)r0.z), otag = (uint32_t)(t + (int)r1.y);
-            if (has_pre && !pref) {
-                issue_loads<2>(vp, ppre, 32, warp, NWARP, 0);
-                __syncwarp();
-                load_pre_weights(kind, r0.w);
-            }
-            if (kind == IK_F4) {
-                if (has_pre) multiply<4, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
-                consume<4, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
-            } else if (kind == IK_F2) {
-                if (has_pre) multiply<2, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
-                consume<2, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
-            } else if (kind == IK_F2CP) {
-                if (has_pre) multiply<2, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
-                consume<2, 1, 3, TR>(acc, v, pon, 48, warp, NWARP, s0, otag, r1.z, 0u, warp * 3, res_s, packed, lane, ck);
+            if (kind == IK_G1) {
+                // first stage of a step: [ctx(t-1) | p2(t)] against the gate tile and the [candidate x-half | z] tile.
+                // Off-chain, loaded here and one after the other (both in flight at once spill registers; prefetched before
+                // A|P2 they delayed OQP's epilogue and the q(t) polls of the attention, H100 80GB HBM3, 700 W): h1(t-1) .
+                // Wg1_h into the gates, then s(t-1) against both tiles.  Both end well before the merged context arrives.
+                if (has_pre) {
+                    issue_loads<2>(vp, ppre, 32, warp, NWARP, 0);
+                    __syncwarp();
+                    load_pre_weights(kind, r0.w);
+                    multiply<4, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
+                    const ItemRec& rec = itab[ii];
+                    const uint64_t* psv = ws + rec.s_base + warp * 64 + lane_w;
+                    issue_loads<2>(vp, psv, 32, warp, NWARP, 0);
+                    __syncwarp();
+                    float wsx[16];
+                    load_weights<4, 2, 2>(wsx, rec.s_w1, rec.s_w2, warp * 2, res_s, packed, lane);
+                    multiply<4, 2, 2, false>(acc, vp, wsx, psv, 32, warp, NWARP, 0, ptag, nullptr);
+                }
+                consume<4, 2, 3, TR>(acc, v, pon, (int)on_nkt, warp, NWARP, s0, otag, r1.z, r1.w, warp * 3, res_s, packed, lane, ck);
             } else {
-                consume<4, 2, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, r1.w, warp * 2, res_s, packed, lane, ck);
+                if (has_pre && !pref) {
+                    issue_loads<2>(vp, ppre, 32, warp, NWARP, 0);
+                    __syncwarp();
+                    load_pre_weights(kind, r0.w);
+                }
+                if (kind == IK_F4) {
+                    if (has_pre) multiply<4, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
+                    consume<4, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
+                } else if (kind == IK_F2) {
+                    if (has_pre) multiply<2, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
+                    consume<2, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
+                } else {
+                    consume<4, 2, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, r1.w, warp * 2, res_s, packed, lane, ck);
+                }
             }
             pref = false;
             // the next stage's off-chain operand is already known: put its loads in flight now, together with those of its
@@ -865,45 +905,73 @@ __global__ void pack_seg_kernel(const float* __restrict__ W, int ldw, int k0, in
     }
 }
 
-// weight-only precompute (double accumulation): C = A . B (+ addv)
-__global__ void matmul_naive_kernel(const float* __restrict__ Amat, int lda, const float* __restrict__ Bmat, int ldb,
-                                    float* __restrict__ Cmat, int ldc, int M, int N, int K, const float* __restrict__ addv) {
-    const int64_t total = (int64_t)M * N;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int m = (int)(i / N), n = (int)(i % N);
-        double a = addv ? (double)addv[n] : 0.0;
-        for (int k = 0; k < K; ++k) a += (double)Amat[(int64_t)m * lda + k] * (double)Bmat[(int64_t)k * ldb + n];
-        Cmat[(int64_t)m * ldc + n] = (float)a;
+// weight-only precompute (double accumulation in k order): C = A . B (+ addv).  One 16 x 16 output tile per 256-thread
+// block, its A and B k-slabs staged in shared memory (the pack runs after every weight update, i.e. every training step)
+__global__ void matmul_f64_kernel(const float* __restrict__ Amat, int lda, const float* __restrict__ Bmat, int ldb,
+                                  float* __restrict__ Cmat, int ldc, int M, int N, int K, const float* __restrict__ addv) {
+    __shared__ float As[16][17], Bs[16][17];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int tiles_n = (N + 15) / 16;
+    const int m = blockIdx.x / tiles_n * 16 + ty, n = blockIdx.x % tiles_n * 16 + tx;
+    double a = (addv && n < N) ? (double)addv[n] : 0.0;
+    for (int k0 = 0; k0 < K; k0 += 16) {
+        As[ty][tx] = (m < M && k0 + tx < K) ? Amat[(int64_t)m * lda + k0 + tx] : 0.f;
+        Bs[ty][tx] = (k0 + ty < K && n < N) ? Bmat[(int64_t)(k0 + ty) * ldb + n] : 0.f;
+        __syncthreads();
+        const int kn = K - k0 < 16 ? K - k0 : 16;
+        for (int k = 0; k < kn; ++k) a += (double)As[ty][k] * (double)Bs[k][tx];
+        __syncthreads();
     }
+    if (m < M && n < N) Cmat[(int64_t)m * ldc + n] = (float)a;
+}
+void matmul_f64(cudaStream_t st, const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K,
+                const float* addv) {
+    matmul_f64_kernel<<<(M + 15) / 16 * ((N + 15) / 16), 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K, addv);
 }
 
 // ---- fused linear stages (weight-only algebra; sums are re-associated, ~1e-6 relative) --------------------------
 //   W_cpF  = [ W_a[80r:80r+256] . W_in[128:384] ; W_in[0:128] ]    [ctx(t-1) | p2(t)] -> z(t)
-//   M1     = W_a[0:80r] . W_in[128:384];  W_sF = W_out . M1;  b_inS = b_out . M1        y(t-1) = s(t-1).W_out + b_out -> z(t)
+//   M1     = W_a[0:80r] . W_in[128:384];  W_sF = W_out . M1;  b_inF = b_in + b_out . M1   y(t-1) = s(t-1).W_out + b_out -> z(t)
 //   W_qp   = [ W_out . W_q | W_out[:, last 80] . W1 ];  b_qF = b_out . W_q;  b_p1F = b_out[last 80] . W1 + b1
-struct FusedTail { int64_t w_cpF, m1, w_sF, w_qp, b_qF, b_p1F, b_inS, total; };
+// z(t) itself is never formed on the chain: the first GRU takes it through
+//   W_g1cp = W_cpF . Wg1_x,  W_g1s = W_sF . Wg1_x           (gates;                       Wg1_x = Wg1[0:256])
+//   W_z1cp = [ W_cpF . Wc1_x | W_cpF ],  W_z1s = [ W_sF . Wc1_x | W_sF ]   ([candidate x-half | z]; Wc1_x = Wc1[0:256])
+// with the biases b_g1F = b_inF . Wg1_x + bg1,  b_z1F = [ b_inF . Wc1_x | b_inF ]  (t > 0) and b_g1F0, b_z1F0: the same with
+// b_in in place of b_inF (t = 0: there is no s(t-1)).  Every product is accumulated in float64 (matmul_f64_kernel).
+// The packed buffer keeps these products only where the kernel reads them: as the MMA fragments of their segments, and the
+// bias vectors in the tail.  The weight products are formed in the regions of the segments whose sources are raw weights
+// (SG_G_H0 .. SG_Y), which are packed last (PackScratch); M1 lives in the tail, whose first 4 x 512 floats then receive the
+// first GRU's folded biases.
+struct FusedTail { int64_t fold, b_qF, b_p1F, b_inF, total; };   // fold: M1 [80r][256], then b_g1F | b_g1F0 | b_z1F | b_z1F0
 FusedTail fused_tail(int r, int64_t slices_total) {
     const int OUT = MF * r;
     FusedTail f;
     int64_t o = (slices_total + 63) / 64 * 64;
-    f.w_cpF = o;  o += (int64_t)(ENC + 128) * U;          // [W_ctxF ; W_in[0:128]]: the on-chain operand [ctx | p2]
-    f.m1 = o;     o += (int64_t)OUT * U;
-    f.w_sF = o;   o += (int64_t)U * U;
-    f.w_qp = o;   o += (int64_t)U * 2 * AU;
+    f.fold = o;   o += (int64_t)OUT * U;                  // >= 4 x 2U floats for every r >= 1
     f.b_qF = o;   o += AU;
     f.b_p1F = o;  o += 256;
-    f.b_inS = o;  o += U;
+    f.b_inF = o;  o += U;
     f.total = o;
     return f;
+}
+struct PackScratch { int64_t w_z1cp, w_z1s, w_g1cp, w_g1s, w_qp, end; };
+PackScratch pack_scratch(const SegDesc* sd) {
+    PackScratch p;
+    int64_t o = sd[SG_G_H0].g_off;
+    p.w_z1cp = o; o += (int64_t)(ENC + 128) * 2 * U;      // [384][512]; columns 256.. hold W_cpF
+    p.w_z1s = o;  o += (int64_t)U * 2 * U;                // [256][512]; columns 256.. hold W_sF
+    p.w_g1cp = o; o += (int64_t)(ENC + 128) * 2 * U;
+    p.w_g1s = o;  o += (int64_t)U * 2 * U;
+    p.w_qp = o;   o += (int64_t)U * 2 * AU;
+    p.end = o;
+    return p;
 }
 
 void build_seg_table(SegDesc* sd, int64_t* total_floats) {
     auto set = [&](int id, int K, int FL, int nw, int kpw) { sd[id].K = K; sd[id].FL = FL; sd[id].nw = nw; sd[id].kpw = kpw; };
-    set(SG_IN_S, 256, 2, 16, 2); set(SG_IN_CP, 384, 2, 16, 3);
-    for (int i = 0; i < 3; ++i) {
-        set(SG_G_H0 + i, 256, 4, 16, 2); set(SG_G_X0 + i, 256, 4, 16, 2);
-        set(SG_C_X0 + i, 256, 2, 16, 2); set(SG_C_RH0 + i, 256, 2, 16, 2);
-    }
+    set(SG_G1_CP, ENC + 128, 4, 16, 3); set(SG_Z1_CP, ENC + 128, 4, 16, 3); set(SG_G1_S, 256, 4, 16, 2); set(SG_Z1_S, 256, 4, 16, 2);
+    for (int i = 0; i < 3; ++i) { set(SG_G_H0 + i, 256, 4, 16, 2); set(SG_C_RH0 + i, 256, 2, 16, 2); }
+    for (int i = 0; i < 2; ++i) { set(SG_G_X1 + i, 256, 4, 16, 2); set(SG_C_X1 + i, 256, 2, 16, 2); }
     set(SG_Y, 256, 4, 16, 2); set(SG_QP, 256, 4, 16, 2); set(SG_PM, MF, 2, 16, 2); set(SG_P2, 256, 2, 8, 4);
     int64_t off = 0;
     for (int s = 0; s < NSEG; ++s) {
@@ -923,8 +991,9 @@ void build_ws_layout(int64_t* buf, int64_t* att, int64_t* total) {
 }
 
 inline int trace_words(int T) { return 16 * (T > 0 ? T : 0) + 16 + 4 * MAX_ITEMS * 8 + 16; }
-// after the trace: the step-0 terms of an initial state, [32][256] (attention vector) + [3][32][512] (GRU states) floats
-constexpr int64_t INIT_Z_FLOATS = (int64_t)BPAD * U, INIT_FLOATS = INIT_Z_FLOATS + 3 * (int64_t)BPAD * 2 * U;
+// after the trace: the step-0 terms of an initial state, [32][512] floats each: init_z, init_zg (attention vector), then
+// [3][32][512] init_g (GRU states)
+constexpr int64_t INIT_ROWS = (int64_t)BPAD * 2 * U, INIT_FLOATS = 5 * INIT_ROWS;
 
 // co-resident CTAs of the forward kernel on the current device (computed once per device; a MIG instance or an H100 PCIe
 // has fewer SMs than the 132 of an H100 SXM).  Also opts the kernel into the full 227 KB of shared memory on that device.
@@ -974,43 +1043,72 @@ extern "C" size_t taco_decoder_workspace_bytes(int B, int Tx, int T, int r) {
 extern "C" int taco_decoder_pack(const taco_decoder_weights* w, int r, float* packed, void* stream) {
     TACO_CHECK(w && packed, "taco_decoder_pack: NULL");
     TACO_CHECK(r >= 1 && MF * r <= 512, "taco_decoder_pack: r=%d out of range (80r <= 512)", r);
-    TACO_CHECK(w->att_Wa && w->in_W && w->out_W && w->att_Wq && w->out_b && w->pre_W1 && w->pre_b1 && w->pre_W2, "taco_decoder_pack: NULL weight");
+    TACO_CHECK(w->att_Wa && w->in_W && w->in_b && w->out_W && w->att_Wq && w->out_b && w->pre_W1 && w->pre_b1 && w->pre_W2,
+               "taco_decoder_pack: NULL weight");
     for (int i = 0; i < 3; ++i) TACO_CHECK(w->gru_Wg[i] && w->gru_Wc[i], "taco_decoder_pack: NULL GRU weight");
+    TACO_CHECK(w->gru_bg[0], "taco_decoder_pack: NULL GRU bias");
     SegDesc sd[NSEG]; int64_t tot;
     build_seg_table(sd, &tot);
     cudaStream_t stm = (cudaStream_t)stream;
     const int OUT = MF * r;
     const int NCY = (OUT + NS - 1) / NS;
     const FusedTail ft = fused_tail(r, tot);
-    float *w_cpF = packed + ft.w_cpF, *m1 = packed + ft.m1, *w_sF = packed + ft.w_sF, *w_qp = packed + ft.w_qp;
+    const PackScratch ps = pack_scratch(sd);
+    TACO_CHECK(ps.end <= sd[SG_QP].g_off, "taco_decoder_pack: scratch overlaps a product segment");
+    float *w_z1cp = packed + ps.w_z1cp, *w_z1s = packed + ps.w_z1s, *m1 = packed + ft.fold, *w_qp = packed + ps.w_qp;
+    float *w_cpF = w_z1cp + U, *w_sF = w_z1s + U, *b_inF = packed + ft.b_inF;      // (row stride 2U)
     const float* w_inA = w->in_W + (int64_t)128 * U;           // W_in[128:384]
-    matmul_naive_kernel<<<256, 256, 0, stm>>>(w->att_Wa + (int64_t)OUT * AU, AU, w_inA, U, w_cpF, U, ENC, U, AU, nullptr);
+    matmul_f64(stm, w->att_Wa + (int64_t)OUT * AU, AU, w_inA, U, w_cpF, 2 * U, ENC, U, AU, nullptr);
     TACO_LAUNCH_CHECK();
-    TACO_CUDA(cudaMemcpyAsync(w_cpF + (int64_t)ENC * U, w->in_W, (size_t)128 * U * sizeof(float), cudaMemcpyDeviceToDevice, stm));
-    matmul_naive_kernel<<<400, 256, 0, stm>>>(w->att_Wa, AU, w_inA, U, m1, U, OUT, U, AU, nullptr);
+    TACO_CUDA(cudaMemcpy2DAsync(w_cpF + (int64_t)ENC * 2 * U, 2 * U * sizeof(float), w->in_W, U * sizeof(float), U * sizeof(float), 128,
+                                cudaMemcpyDeviceToDevice, stm));
+    matmul_f64(stm, w->att_Wa, AU, w_inA, U, m1, U, OUT, U, AU, nullptr);
     TACO_LAUNCH_CHECK();
-    matmul_naive_kernel<<<256, 256, 0, stm>>>(w->out_W, OUT, m1, U, w_sF, U, U, U, OUT, nullptr);
+    matmul_f64(stm, w->out_W, OUT, m1, U, w_sF, 2 * U, U, U, OUT, nullptr);
     TACO_LAUNCH_CHECK();
-    matmul_naive_kernel<<<1, 256, 0, stm>>>(w->out_b, OUT, m1, U, packed + ft.b_inS, U, 1, U, OUT, nullptr);
+    matmul_f64(stm, w->out_b, OUT, m1, U, b_inF, U, 1, U, OUT, w->in_b);
     TACO_LAUNCH_CHECK();
-    matmul_naive_kernel<<<256, 256, 0, stm>>>(w->out_W, OUT, w->att_Wq, AU, w_qp, 2 * AU, U, AU, OUT, nullptr);
+    // the first GRU's products of z: gates (. Wg1_x) and candidate x-half (. Wc1_x), weights and biases
+    const float *wg1x = w->gru_Wg[0], *wc1x = w->gru_Wc[0];
+    matmul_f64(stm, w_cpF, 2 * U, wg1x, 2 * U, packed + ps.w_g1cp, 2 * U, ENC + 128, 2 * U, U, nullptr);
     TACO_LAUNCH_CHECK();
-    matmul_naive_kernel<<<256, 256, 0, stm>>>(w->out_W + (OUT - MF), OUT, w->pre_W1, 256, w_qp + AU, 2 * AU, U, 256, MF, nullptr);
+    matmul_f64(stm, w_sF, 2 * U, wg1x, 2 * U, packed + ps.w_g1s, 2 * U, U, 2 * U, U, nullptr);
     TACO_LAUNCH_CHECK();
-    matmul_naive_kernel<<<1, 256, 0, stm>>>(w->out_b, OUT, w->att_Wq, AU, packed + ft.b_qF, AU, 1, AU, OUT, nullptr);
+    matmul_f64(stm, w_cpF, 2 * U, wc1x, U, w_z1cp, 2 * U, ENC + 128, U, U, nullptr);
     TACO_LAUNCH_CHECK();
-    matmul_naive_kernel<<<1, 256, 0, stm>>>(w->out_b + (OUT - MF), MF, w->pre_W1, 256, packed + ft.b_p1F, 256, 1, 256, MF, w->pre_b1);
+    matmul_f64(stm, w_sF, 2 * U, wc1x, U, w_z1s, 2 * U, U, U, U, nullptr);
+    TACO_LAUNCH_CHECK();
+    const float* zb[2] = {b_inF, w->in_b};                     // z's bias at t > 0 and at t = 0
+    const int64_t gdst[2] = {ft.fold, ft.fold + 2 * U}, zdst[2] = {ft.fold + 4 * U, ft.fold + 6 * U};   // M1 is consumed
+    for (int i = 0; i < 2; ++i) {
+        matmul_f64(stm, zb[i], U, wg1x, 2 * U, packed + gdst[i], 2 * U, 1, 2 * U, U, w->gru_bg[0]);
+        TACO_LAUNCH_CHECK();
+        matmul_f64(stm, zb[i], U, wc1x, U, packed + zdst[i], U, 1, U, U, nullptr);
+        TACO_LAUNCH_CHECK();
+        TACO_CUDA(cudaMemcpyAsync(packed + zdst[i] + U, zb[i], U * sizeof(float), cudaMemcpyDeviceToDevice, stm));
+    }
+    matmul_f64(stm, w->out_W, OUT, w->att_Wq, AU, w_qp, 2 * AU, U, AU, OUT, nullptr);
+    TACO_LAUNCH_CHECK();
+    matmul_f64(stm, w->out_W + (OUT - MF), OUT, w->pre_W1, 256, w_qp + AU, 2 * AU, U, 256, MF, nullptr);
+    TACO_LAUNCH_CHECK();
+    matmul_f64(stm, w->out_b, OUT, w->att_Wq, AU, packed + ft.b_qF, AU, 1, AU, OUT, nullptr);
+    TACO_LAUNCH_CHECK();
+    matmul_f64(stm, w->out_b + (OUT - MF), MF, w->pre_W1, 256, packed + ft.b_p1F, 256, 1, 256, MF, w->pre_b1);
     TACO_LAUNCH_CHECK();
 
     struct Src { const float* W; int ld; int k0; };
     Src src[NSEG];
-    src[SG_IN_S] = {w_sF, U, 0}; src[SG_IN_CP] = {w_cpF, U, 0};
+    src[SG_G1_CP] = {packed + ps.w_g1cp, 2 * U, 0}; src[SG_Z1_CP] = {w_z1cp, 2 * U, 0};
+    src[SG_G1_S] = {packed + ps.w_g1s, 2 * U, 0};   src[SG_Z1_S] = {w_z1s, 2 * U, 0};
     for (int i = 0; i < 3; ++i) {
-        src[SG_G_X0 + i] = {w->gru_Wg[i], 2 * U, 0};  src[SG_G_H0 + i] = {w->gru_Wg[i], 2 * U, U};     // rows: x then h (TF 1.2 GRUCell)
-        src[SG_C_X0 + i] = {w->gru_Wc[i], U, 0};      src[SG_C_RH0 + i] = {w->gru_Wc[i], U, U};
+        src[SG_G_H0 + i] = {w->gru_Wg[i], 2 * U, U};  src[SG_C_RH0 + i] = {w->gru_Wc[i], U, U};    // rows: x then h (TF 1.2 GRUCell)
     }
+    for (int i = 1; i < 3; ++i) { src[SG_G_X1 + i - 1] = {w->gru_Wg[i], 2 * U, 0}; src[SG_C_X1 + i - 1] = {w->gru_Wc[i], U, 0}; }
     src[SG_Y] = {w->out_W, OUT, 0}; src[SG_QP] = {w_qp, 2 * AU, 0}; src[SG_PM] = {w->pre_W1, 256, 0}; src[SG_P2] = {w->pre_W2, 128, 0};
-    for (int s = 0; s < NSEG; ++s) {
+    // the segments made from the products first: the others overwrite the scratch the products were formed in
+    const int order[NSEG] = {SG_G1_CP, SG_Z1_CP, SG_G1_S, SG_Z1_S, SG_QP, SG_G_H0, SG_G_H1, SG_G_H2, SG_G_X1, SG_G_X2,
+                             SG_C_X1, SG_C_X2, SG_C_RH0, SG_C_RH1, SG_C_RH2, SG_Y, SG_PM, SG_P2};
+    for (int s : order) {
         const int64_t total = (int64_t)NS * sd[s].slice_floats;
         const int blocks = (int)((total + 255) / 256);
         pack_seg_kernel<<<blocks, 256, 0, stm>>>(src[s].W, src[s].ld, src[s].k0, sd[s].K, sd[s].FL, sd[s].nw, sd[s].kpw, s, NCY, OUT, packed + sd[s].g_off);
@@ -1051,21 +1149,25 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     P.NCY = (P.OUT + NS - 1) / NS;
     P.Tq = (a->Tx + 3) / 4;            // quarter width; the last quarter is ragged when Tx % 4 != 0
     TACO_CHECK(P.Tq <= 64 && P.NCY <= 16, "taco_decoder_fwd: Tx/4 = %d > 64 or 80r/32 > 16", P.Tq);
-    P.in_b = W.in_b; P.out_b = W.out_b; P.pre_b1 = W.pre_b1; P.pre_b2 = W.pre_b2; P.att_v = W.att_v;
+    P.out_b = W.out_b; P.pre_b1 = W.pre_b1; P.pre_b2 = W.pre_b2; P.att_v = W.att_v;
     for (int i = 0; i < 3; ++i) { P.gru_bg[i] = W.gru_bg[i]; P.gru_bc[i] = W.gru_bc[i]; }
     const FusedTail ft = fused_tail(a->r, tot);
-    P.b_qF = a->packed + ft.b_qF; P.b_p1F = a->packed + ft.b_p1F; P.b_inS = a->packed + ft.b_inS;
+    P.b_qF = a->packed + ft.b_qF; P.b_p1F = a->packed + ft.b_p1F;
+    P.b_g1F = a->packed + ft.fold; P.b_g1F0 = P.b_g1F + 2 * U; P.b_z1F = P.b_g1F + 4 * U; P.b_z1F0 = P.b_g1F + 6 * U;
 
     // ---- the per-step program: one record per stage ----
     int n = 0;
     auto stage = [&](int kind, int st_id, int pre_seg, int pre_src, int pre_tagd, int pre_skip0, int on_seg, int on_seg2, int on_src, int on_tagd, int on_s0) {
         P.items[n++] = Item{kind, st_id, pre_seg, pre_src, pre_tagd, pre_skip0, on_seg, on_seg2, on_src, on_tagd, on_s0};
     };
-    stage(IK_F2CP, ST_IN, SG_IN_S, B_S, 0, 1, SG_IN_CP, -1, B_CP, 1, 2);         // s(t-1) | [ctx(t-1) | p2(t)] (no s, no context at t = 0)
-    for (int i = 0; i < 3; ++i) {
-        const int x = (i == 0) ? B_Z : B_H0 + (i - 1);
-        stage(IK_F4, ST_G0 + i, SG_G_H0 + i, B_H0 + i, 0, 1, SG_G_X0 + i, -1, x, 1, 0);           // h_i(t-1) | x
-        stage(IK_F2, ST_C0 + i, SG_C_X0 + i, x, 1, 0, SG_C_RH0 + i, -1, B_RH0 + i, 1, 0);         // x (already consumed by the gates) | r*h
+    // G1: h1(t-1) (and s(t-1), see ItemRec) | [ctx(t-1) | p2(t)] against the gate and [candidate x-half | z] tiles (no h, no
+    // s, no context at t = 0); C1: r*h only, its x-half came with G1
+    stage(IK_G1, ST_G0, SG_G_H0, B_H0, 0, 1, SG_G1_CP, SG_Z1_CP, B_CP, 1, 2);
+    stage(IK_F2, ST_C0, -1, 0, 0, 0, SG_C_RH0, -1, B_RH0, 1, 0);
+    for (int i = 1; i < 3; ++i) {
+        const int x = B_H0 + (i - 1);
+        stage(IK_F4, ST_G0 + i, SG_G_H0 + i, B_H0 + i, 0, 1, SG_G_X1 + i - 1, -1, x, 1, 0);       // h_i(t-1) | x
+        stage(IK_F2, ST_C0 + i, SG_C_X1 + i - 1, x, 1, 0, SG_C_RH0 + i, -1, B_RH0 + i, 1, 0);     // x (already consumed by the gates) | r*h
     }
     if (a->mode != TACO_DEC_INFER) stage(IK_PM, ST_PM, -1, 0, 0, 0, -1, -1, 0, 0, 0);             // teacher frame t+1 -> p1m(t+1), off-chain
     stage(IK_F4X2, ST_OQP, -1, 0, 0, 0, SG_Y, SG_QP, B_S, 1, 0);
@@ -1074,7 +1176,7 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
 
     // ---- residency: on-chain segments in shared memory, off-chain segments read from the packed buffer (L2); when the
     //      keys/values leave too little shared memory (large Tx) further segments are read from L2 as well ----
-    int off = 16 + 6400 + 512 + 384 + 256 + 704 + 1024 + 64 + 256;
+    int off = 16 + 6400 + 512 + 384 + 256 + 704 + 256;
     off = (off + 31) / 32 * 32;
     P.smem_kv_off = off;
     off += P.Tq * KV_LD + P.Tq * ENC;
@@ -1082,7 +1184,8 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     P.smem_res_off = off;
     const int budget = (227 * 1024) / 4 - off;
     // (build_seg_table leaves every segment in L2; the packed buffer is far below the 2^31 floats a weight word can address)
-    const int sm_order[] = {SG_IN_CP, SG_G_X0, SG_C_RH0, SG_G_X1, SG_C_RH1, SG_G_X2, SG_C_RH2, SG_QP, SG_Y, SG_P2};
+    // (at Tx = 128 every slice but the output tile SG_Y fits; SG_Y is loaded with OQP's operand, in the shadow of its hop)
+    const int sm_order[] = {SG_G1_CP, SG_Z1_CP, SG_C_RH0, SG_G_X1, SG_C_RH1, SG_G_X2, SG_C_RH2, SG_QP, SG_Y, SG_P2};
     int res = 0;
     for (int s : sm_order) {
         if (P.seg[s].slice_floats <= budget - res) { P.seg[s].smem_off = res; res += P.seg[s].slice_floats; }
@@ -1114,30 +1217,36 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     cfg.attrs = &coop; cfg.numAttrs = 1;
     TACO_CUDA(cudaMemsetAsync(a->workspace, 0, (size_t)ws_total * 8, st));
     // initial state (speaker-conditioned decoder): the kernel skips the h(t-1) and attention products at t = 0, so their
-    // step-0 values att0 . W_in[128:] and h0_i . Wg_i[256:] are formed here, per row of this launch, and added by the IN
-    // and G epilogues of step 0 (the C stage sees h0 through r * h and the state update)
+    // step-0 values are formed here, per row of this launch, and added by the G1 and G epilogues of step 0 (the C stage
+    // sees h0 through r * h and the state update): with iz = att0 . W_in[128:], init_z = [iz . Wc1_x | iz] and
+    // init_zg = iz . Wg1_x (z and the first GRU's products of it), init_g = h0_i . Wg_i[256:]
     if (a->att0 || a->h0) {
         float* init = reinterpret_cast<float*>(reinterpret_cast<uint64_t*>(a->workspace) + ws_total + trace_words(a->T));
         const int RS = P.a.row_stride;
-        auto term = [&](const float* X, const float* Wm, int N, float* dst) {     // dst[b][n] = X[b] . Wm[:, n], b < B
-            taco_gemm_desc g;                                                   // (the library's own GEMM)
+        // dst[b][n] = X[b] . Wm[:, n], b < B (the library's own GEMM)
+        auto term = [&](const float* X, int64_t ldx, const float* Wm, int N, float* dst) {
+            taco_gemm_desc g;
             memset(&g, 0, sizeof(g));
-            g.A = X; g.lda = U; g.B = Wm; g.ldb = N; g.C = dst; g.ldc = N; g.M = a->B; g.N = N; g.K = U;
+            g.A = X; g.lda = ldx; g.B = Wm; g.ldb = N; g.C = dst; g.ldc = 2 * U; g.M = a->B; g.N = N; g.K = U;
             g.taps = 1; g.batch = 1;
             return taco_gemm(&g, stream);
         };
         if (a->att0) {
-            TACO_CHECK(W.in_W != nullptr, "taco_decoder_fwd: att0 needs weights->in_W");
-            if (term(a->att0 + (int64_t)a->row0 * U, W.in_W + (int64_t)128 * U, U, init)) return 1;
-            P.init_z = init;
+            TACO_CHECK(W.in_W != nullptr && W.gru_Wg[0] != nullptr && W.gru_Wc[0] != nullptr,
+                       "taco_decoder_fwd: att0 needs weights->in_W, gru_Wg[0] and gru_Wc[0]");
+            float *iz = init + U, *izg = init + INIT_ROWS;
+            if (term(a->att0 + (int64_t)a->row0 * U, U, W.in_W + (int64_t)128 * U, U, iz)) return 1;
+            if (term(iz, 2 * U, W.gru_Wc[0], U, init)) return 1;
+            if (term(iz, 2 * U, W.gru_Wg[0], 2 * U, izg)) return 1;
+            P.init_z = init; P.init_zg = izg;
         }
         if (a->h0) {
             for (int i = 0; i < 3; ++i) {
                 TACO_CHECK(W.gru_Wg[i] != nullptr, "taco_decoder_fwd: h0 needs weights->gru_Wg");
-                if (term(a->h0 + ((int64_t)i * RS + a->row0) * U, W.gru_Wg[i] + (int64_t)U * 2 * U, 2 * U,
-                         init + INIT_Z_FLOATS + (int64_t)i * BPAD * 2 * U)) return 1;
+                if (term(a->h0 + ((int64_t)i * RS + a->row0) * U, U, W.gru_Wg[i] + (int64_t)U * 2 * U, 2 * U,
+                         init + (2 + i) * INIT_ROWS)) return 1;
             }
-            P.init_g = init + INIT_Z_FLOATS;
+            P.init_g = init + 2 * INIT_ROWS;
         }
     }
     static const bool trace_build = getenv("TACO_TRACE") != nullptr;     // per-stage clock trace (scripts/dec_time.py)
