@@ -200,7 +200,8 @@ extern "C" int taco_bigru_trace_read(long long* dst) {     // TRACE_STEPS x TRAC
 extern "C" int taco_bigru_fwd_h0(const float* xp, const float* Wg_h_fw, const float* Wc_h_fw, const float* Wg_h_bw,
                                  const float* Wc_h_bw, const float* h0_fw, const float* h0_bw, float* out, int B, int T,
                                  void* stream) {
-    TACO_CHECK(xp && Wg_h_fw && Wc_h_fw && Wg_h_bw && Wc_h_bw && out, "taco_bigru_fwd: NULL pointer");
+    // the operands of an empty sequence may be NULL (torch's empty tensors have no storage); the weights never may
+    TACO_CHECK(Wg_h_fw && Wc_h_fw && Wg_h_bw && Wc_h_bw && ((xp && out) || (int64_t)B * T == 0), "taco_bigru_fwd: NULL pointer");
     TACO_CHECK(B >= 0 && T >= 0, "taco_bigru_fwd: negative size");
     TACO_CHECK((int64_t)B * T * 768 < (int64_t)1 << 31, "taco_bigru_fwd: B*T = %lld too large for 32-bit offsets", (long long)B * T);
     if (B == 0 || T == 0) return 0;

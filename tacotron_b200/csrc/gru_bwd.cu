@@ -144,7 +144,9 @@ bigru_bwd_kernel(float* __restrict__ dxp, const float* __restrict__ dOut, const 
 extern "C" int taco_bigru_bwd_h0(float* dxp, const float* dOut, const float* out, const float* ACT, const float* Wg_h_fw,
                                  const float* Wc_h_fw, const float* Wg_h_bw, const float* Wc_h_bw, const float* h0_fw,
                                  const float* h0_bw, float* dh0, int B, int T, void* stream) {
-    TACO_CHECK(dxp && dOut && out && ACT && Wg_h_fw && Wc_h_fw && Wg_h_bw && Wc_h_bw, "taco_bigru_bwd: NULL pointer");
+    // the operands of an empty sequence may be NULL (torch's empty tensors have no storage); the weights never may
+    TACO_CHECK(Wg_h_fw && Wc_h_fw && Wg_h_bw && Wc_h_bw && ((dxp && dOut && out && ACT) || (int64_t)B * T == 0),
+               "taco_bigru_bwd: NULL pointer");
     TACO_CHECK(B >= 0 && T >= 0, "taco_bigru_bwd: negative size");
     if (B == 0 || (T == 0 && !dh0)) return 0;             // T == 0 with dh0: the kernel only writes dh0 = 0
     TACO_LAUNCH(bigru_bwd_kernel, dim3(B, 2), 512, 0, (cudaStream_t)stream, dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw,

@@ -16,14 +16,14 @@ def bigru_bwd_h0(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw,
     B, T, _ = out.shape
     Hn = 128
     for d, (Wg, Wc, h0) in enumerate(((Wg_h_fw, Wc_h_fw, h0_fw), (Wg_h_bw, Wc_h_bw, h0_bw))):
-        carry = torch.zeros(B, Hn, dtype=out.dtype)
+        carry = torch.zeros(B, Hn, dtype=out.dtype, device=out.device)
         order = range(T - 1, -1, -1) if d == 0 else range(T)
         for t in order:
             tp = t - 1 if d == 0 else t + 1
             if 0 <= tp < T:
                 hprev = out[:, tp, d * Hn:(d + 1) * Hn]
             else:
-                hprev = h0 if h0 is not None else torch.zeros(B, Hn, dtype=out.dtype)
+                hprev = h0 if h0 is not None else torch.zeros(B, Hn, dtype=out.dtype, device=out.device)
             a = ACT[:, t, d * 384:(d + 1) * 384]
             r, u, c = a[:, :Hn], a[:, Hn:2 * Hn], a[:, 2 * Hn:]
             dh = dOut[:, t, d * Hn:(d + 1) * Hn] + carry
@@ -43,7 +43,7 @@ def bigru_fwd_h0(out, xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw):
     B, T, _ = out.shape
     Hn = 128
     for d, (Wg, Wc, h0) in enumerate(((Wg_h_fw, Wc_h_fw, h0_fw), (Wg_h_bw, Wc_h_bw, h0_bw))):
-        h = h0 if h0 is not None else torch.zeros(B, Hn, dtype=out.dtype)
+        h = h0 if h0 is not None else torch.zeros(B, Hn, dtype=out.dtype, device=out.device)
         for t in (range(T) if d == 0 else range(T - 1, -1, -1)):
             x = xp[:, t, d * 384:(d + 1) * 384]
             g = torch.sigmoid(x[:, :2 * Hn] + h @ Wg)
