@@ -196,6 +196,10 @@ typedef struct taco_decoder_weights {   /* all TF layout, device pointers */
 /* bytes of the packed-weight buffer / of the workspace taco_decoder_fwd needs */
 size_t taco_decoder_packed_bytes(int r);
 size_t taco_decoder_workspace_bytes(int B, int Tx, int T, int r);
+/* 64-bit word offset in that workspace of the per-stage trace the TACO_TRACE build writes (scripts/dec_time.py): from
+ * there [16 T + 16] words of %globaltimer stamps of CTA 0, one per finished stage, then [4][20][8] clock64 records of
+ * the stages of steps 10..13                                                                                          */
+int64_t taco_decoder_trace_offset(void);
 /* re-lay the weights per CTA column slice (call once per weight update) */
 int taco_decoder_pack(const taco_decoder_weights* w, int r, float* packed, void* stream);
 
@@ -227,6 +231,12 @@ typedef struct taco_decoder_args {
                                     this launch's row b is row0 + b), or NULL = zero state (cell.zero_state)  */
     const float*   att0;         /* [row_stride][256] initial attention vector, or NULL = zero; needs weights->in_W
                                     (h0 needs weights->gru_Wg): their step-0 products are formed in the workspace */
+    int32_t        win_back;     /* attention window (TACO_DEC_INFER only; win_ahead = 0: no window, the default).  With   */
+    int32_t        win_ahead;    /* p(-1) = 0 and N_b = min(text_length_b, Tx), step t scores only the positions j with
+                                    max(0, p(t-1) - win_back) <= j <= p(t-1) + win_ahead, j < N_b (the others are -inf
+                                    before the softmax); p(t) = the lowest j of highest score.  win_back >= 0,
+                                    win_ahead >= 1; bounds >= Tx - 1 allow every position and give the unwindowed bits */
+    int32_t*       peak;         /* [B][T] p(t) of each step (indexed like align), or NULL; needs the window          */
 } taco_decoder_args;
 
 int taco_decoder_fwd(const taco_decoder_args* a, void* stream);

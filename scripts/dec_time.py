@@ -1,17 +1,21 @@
 """Time only the decoder section of the C2 step (quick A/B of decoder variants).
 
-    TACO_TRACE=1 python scripts/dec_time.py [--precision fp32x3|tf32|fp32]
+    TACO_TRACE=1 python scripts/dec_time.py [--precision fp32x3|tf32|fp32] [--window BACK,AHEAD]
 
-With TACO_TRACE set, the traced kernel instantiation also records per-slot and per-phase clocks of CTA 0."""
+With TACO_TRACE set, the traced kernel instantiation also records per-slot and per-phase clocks of CTA 0; --window
+times the decoder with that attention window (Config.attention_window)."""
 import argparse, os, sys, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from tacotron_b200 import Config, Tacotron
 ap = argparse.ArgumentParser()
 ap.add_argument("--precision", default="fp32x3", choices=["fp32x3", "tf32", "fp32"], help="default: the benchmark's mode")
+ap.add_argument("--window", default=None, help="attention window BACK,AHEAD (default: none)")
 args = ap.parse_args()
+window = None if args.window is None else tuple(int(v) for v in args.window.split(","))
 B, TX, T, R = 32, 128, 200, 5
-m = Tacotron(Config(r=R, vocab_size=64, max_decode_iter=T, precision=args.precision), None, train=False, seed=1)
+m = Tacotron(Config(r=R, vocab_size=64, max_decode_iter=T, precision=args.precision, attention_window=window), None,
+             train=False, seed=1)
 g = torch.Generator().manual_seed(0)
 inp = {"text": torch.randint(1, 64, (B, TX), generator=g, dtype=torch.int32).cuda(), "text_length": torch.full((B,), TX, dtype=torch.int32).cuda()}
 m.step_ns = torch.zeros(T, dtype=torch.int64, device="cuda")
@@ -25,15 +29,16 @@ for _ in range(5):
     tt = dict(m._marks); m._marks = None
     dec.append(tt["encoder"].elapsed_time(tt["decoder"]))
 ns = m.step_ns.cpu().numpy()
-print("precision", args.precision, "decoder ms", statistics.median(dec), "step p50 us", float(statistics.median(((ns[1:]-ns[:-1])/1e3).tolist())))
+print("precision", args.precision, "window", window, "decoder ms", statistics.median(dec), "step p50 us", float(statistics.median(((ns[1:]-ns[:-1])/1e3).tolist())))
 if os.environ.get("TACO_TRACE"):
     import numpy as np
+    from tacotron_b200 import _lib as L
     ws = m.runtime.dec_ws.view(torch.int64).cpu().numpy()
-    total = (10 * 32 + 48) * 4 * 64             # exchange buffers [4 row groups][nkt][8][8] words (decoder.cu build_ws_layout)
-    total += 32 * 2 * 4 * (2 + 256)             # + attention exchange [32 utterances][2][4] x (2 statistics + 256 context words)
+    total = int(L.lib().taco_decoder_trace_offset())   # where the trace starts in the workspace (decoder.cu build_ws_layout)
     names = ["G1", "C1", "G2", "C2", "G3", "C3", "OQP", "A|P2"]
     n = 1 + len(names) * T
     tr = ws[total: total + n]
+    assert (tr > 0).all() and (np.diff(tr) >= 0).all(), "the trace is not where taco_decoder_trace_offset says"
     d = np.diff(tr)                              # d[i] = time of entry i+1 - entry i; entry 0 = prologue
     d = d[: (len(d) // len(names)) * len(names)].reshape(-1, len(names))[5:]
     med = np.median(d, axis=0)

@@ -72,6 +72,7 @@ class DecoderArgs(C.Structure):
         ("h_save", C.c_void_p),
         ("row0", C.c_int32), ("row_stride", C.c_int32), ("max_ctas", C.c_int32),
         ("h0", C.c_void_p), ("att0", C.c_void_p),
+        ("win_back", C.c_int32), ("win_ahead", C.c_int32), ("peak", C.c_void_p),
     ]
 
 
@@ -113,7 +114,8 @@ EXPORTS = [
     "taco_last_error", "taco_version", "taco_device_info", "taco_linear_fwd", "taco_linear_route", "taco_pack_weight",
     "taco_pack_weight_x3", "taco_highway_stack_fwd",
     "taco_maxpool_fwd", "taco_gather_rows", "taco_mask_rows", "taco_bigru_fwd", "taco_bigru_fwd_h0",
-    "taco_decoder_packed_bytes", "taco_decoder_workspace_bytes", "taco_decoder_pack", "taco_decoder_fwd",
+    "taco_decoder_packed_bytes", "taco_decoder_workspace_bytes", "taco_decoder_trace_offset", "taco_decoder_pack",
+    "taco_decoder_fwd",
     "taco_decoder_capacity",
     "taco_l1_loss_fwd", "taco_l1_partial_count", "taco_launch_count",
     # training path
@@ -167,6 +169,8 @@ def lib():
     L.taco_decoder_packed_bytes.restype = C.c_size_t
     L.taco_decoder_workspace_bytes.argtypes = [C.c_int] * 4
     L.taco_decoder_workspace_bytes.restype = C.c_size_t
+    L.taco_decoder_trace_offset.argtypes = []
+    L.taco_decoder_trace_offset.restype = C.c_int64
     L.taco_decoder_pack.argtypes = [C.POINTER(DecoderWeights), C.c_int, C.c_void_p, C.c_void_p]
     L.taco_decoder_fwd.argtypes = [C.POINTER(DecoderArgs), C.c_void_p]
     L.taco_decoder_capacity.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_int)]

@@ -51,6 +51,12 @@
 //     built on, fewer than the 32 this grid needs; the count depends on each die's GPC configuration.)
 //     tanh(k+q) = 1 - 2/(e^{2k} e^{2q} + 1) with e^{2k} precomputed once and e^{2q} once per step: one MUFU per
 //     element instead of two.
+//   * attention window (opt-in, free-running decoding; decoder_kernel<.., WIN = true>): the score write masks positions
+//     outside [p(t-1) - back, p(t-1) + ahead]; warp 4 publishes its quarter's lowest maximising position as one more
+//     {value, tag} word after its partial context, and at the start of step t+1's attention thread 128 combines the
+//     four (lowest quarter holding the utterance's max) beside the q(t+1) polls, so no new exchange sits on the chain
+//     (the windowed step still measures ~0.3 us longer, DESIGN.md 3.4).  The off instantiation is the plain kernel,
+//     instruction for instruction.
 //
 // Unchanged from v3: grid = 32 co-resident CTAs per row group of 8 utterances (128 = 4 row groups when the device holds
 // them), CTA (rg, cs) owns utterance rows 8rg..8rg+7 and the
@@ -125,6 +131,7 @@ struct DecParams {
     int n_items;
     int64_t buf[NBUF];           // word offsets of the exchange buffers
     int64_t att_off;             // word offset of the attention exchange region
+    int64_t peak_off;            // word offset of the attention window's peak words
     int64_t trace_off;
     taco_decoder_args a;
     const float *gru_bg[3], *gru_bc[3], *out_b, *pre_b1, *pre_b2, *att_v;
@@ -309,7 +316,10 @@ struct ItemRec { uint32_t flags, pre_base; int pre_tagd; uint32_t pre_w; uint32_
 // flags: kind | stage << 8 | has_pre << 16 | pre_skip0 << 17 | on_s0 << 20
 // s_*: the second off-chain operand of the G1 item, s(t-1), and its two weight tiles (SG_G1_S, SG_Z1_S)
 
-template <bool TR>     // TR: per-stage clock64 trace of CTA 0 (scripts/dec_time.py); the production instantiation has none of it
+// TR: per-stage clock64 trace of CTA 0 (scripts/dec_time.py); the production instantiation has none of it.
+// WIN: attention window (taco_decoder_args win_back / win_ahead, free-running decoding only): the scores outside
+// [p(t-1) - back, p(t-1) + ahead] are masked and each step's peak p(t) is found; without it the kernel is the plain one.
+template <bool TR, bool WIN>
 __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant__ DecParams P) {
     extern __shared__ __align__(16) float smem[];
     // smem map (floats): [0,16) reserved | part 6400 | part2 512 | loc 384 | bias 256 | att 704 | itab 256 | kv | weights
@@ -319,6 +329,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     float* loc_s = part2_s + 512;                                 // h_loc[3][64] | u_loc[64] | z_loc[64] | cx_loc[64]
     float* bias_s = loc_s + 384;                                  // [NBR][16]
     float* att_s = bias_s + 256;                                  // eq[256] | v[256] | e[64] | p[64] | misc[64]
+                                                                  // (misc: V0 | p(t-1) of the window)
     ItemRec* itab = reinterpret_cast<ItemRec*>(att_s + 704);                 // [MAX_ITEMS] resolved stage records (20 x 12 words)
     uint32_t* otab = reinterpret_cast<uint32_t*>(itab + MAX_ITEMS);          // [NOUT] output word offsets of this CTA
     float* ek_s = smem + P.smem_kv_off;
@@ -497,6 +508,37 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     const int e_row = row0 + e_brow;
     const int e_word = e_brow * 8 + perm8(e_wc);             // word inside this CTA's k-tile block of an exchange buffer
 
+    // ---- attention window: the peak p(ts) of step ts from the four quarters' {max, sum} and peak words (the lowest
+    //      quarter whose max is the utterance's, then that quarter's lowest maximising position; p(ts - 1) when every
+    //      score is masked).  Read a whole step after they were published, so the poll normally finds them there ----
+    // this utterance's peak words [2 parity][4 quarters] {position, tag} (formed at each use: a pointer kept live across
+    // the kernel costs the windowed instantiation a spill)
+    auto xpeak = [&]() { return ws + P.peak_off + (int64_t)arow * (2 * 4); };
+    auto window_peak = [&](int ts, int pprev) {
+        const uint32_t tag = (uint32_t)ts + 1;
+        const uint64_t* xs = ws + P.att_off + (int64_t)arow * (2 * 4 * 2) + (ts & 1) * 4 * 2;
+        const uint64_t* xk = xpeak() + (ts & 1) * 4;
+        ulonglong2 sw[4];
+        uint64_t kw[4];
+#pragma unroll
+        for (int qd = 0; qd < 4; ++qd) { sw[qd] = ll_load2(xs + qd * 2); kw[qd] = ll_load1(xk + qd); }
+        float mq[4], M = -INFINITY;
+#pragma unroll
+        for (int qd = 0; qd < 4; ++qd) {
+            ll_spin(sw[qd], xs + qd * 2, tag);
+            mq[qd] = __uint_as_float((uint32_t)sw[qd].x);
+            M = fmaxf(M, mq[qd]);
+        }
+        int p = pprev;
+        bool found = false;
+#pragma unroll
+        for (int qd = 0; qd < 4; ++qd) {
+            const int pk = __float_as_int(ll_spin1(kw[qd], xk + qd, tag));
+            if (!found && M > -INFINITY && mq[qd] == M) { p = pk; found = true; }
+        }
+        return p;
+    };
+
     // ---- attention of step t on warps 0..7 (256 threads): scores, partial softmax / context, merge of the quarters ----
     auto attention = [&](int t) {
         const uint32_t tag = (uint32_t)t + 1;
@@ -511,6 +553,10 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             const int k0 = ((tid >> 2) << 3) + (tid & 3);        // physical pair (2p, 2p+1) = logical k0, k0+4
             eq_s[k0] = exp2x(qq.x);
             eq_s[k0 + 4] = exp2x(qq.y);
+        } else if (WIN && tid == 128) {   // p(t-1), off the chain: its words are a step old, the poll runs beside q(t)'s
+            const int pp = (t > 0) ? window_peak(t - 1, __float_as_int(misc_s[1])) : 0;
+            misc_s[1] = __int_as_float(pp);
+            if (t > 0 && aq == 0 && A.peak) A.peak[(int64_t)arow * T + t - 1] = pp;
         }
         if (TR && cktr) cktr[0] = clock64();
         named_bar(1, 256);
@@ -525,6 +571,12 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
                 vv[0] = v0.x; vv[1] = v0.y; vv[2] = v0.z; vv[3] = v0.w; vv[4] = v1.x; vv[5] = v1.y; vv[6] = v1.z; vv[7] = v1.w;
             }
             const float V0 = misc_s[0];
+            int wlo = 0, whi = my_len - 1;              // allowed positions (WIN); the host keeps back, ahead <= Tx
+            if (WIN) {
+                const int pp = __float_as_int(misc_s[1]);
+                wlo = max(pp - A.win_back, 0);
+                whi = min(pp + A.win_ahead, min(my_len, Tx) - 1);
+            }
             for (int jb = 0; jb < Tq; jb += 32) {       // 4 positions per warp and round
                 float a4[4];
 #pragma unroll
@@ -563,7 +615,10 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
                 b1 += __shfl_xor_sync(0xffffffffu, b1, 1);
                 const int jj = ((lane >> 4) & 1) * 2 + ((lane >> 3) & 1);
                 const int j = jb + warp + 8 * jj;
-                if ((lane & 7) == 0 && j < Tq) e_s[j] = ((int)aq * Tq + j < my_len) ? fmaf(-2.0f, b1, V0) : -INFINITY;
+                if ((lane & 7) == 0 && j < Tq) {
+                    const int jg = (int)aq * Tq + j;
+                    e_s[j] = (WIN ? (jg >= wlo && jg <= whi) : jg < my_len) ? fmaf(-2.0f, b1, V0) : -INFINITY;
+                }
             }
         }
         if (TR && cktr) cktr[2] = clock64();
@@ -601,6 +656,13 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             }
             if (Tq & 1) c0 = fmaf(p_s[Tq - 1], vals_s[(Tq - 1) * ENC + tid], c0);
             ll_store(xctx + (xp * 4 + aq) * ENC + tid, c0 + c1, tag);
+        }
+        if (WIN && warp == 4) {                          // this quarter's peak: its lowest position holding the max (done
+            const bool h0 = lane < Tq && e_s[lane] == m;  // after warp 4's partial context, so nothing waits for it)
+            const bool h1 = lane + 32 < Tq && e_s[lane + 32] == m;
+            const uint32_t b0 = __ballot_sync(0xffffffffu, h0), b1 = __ballot_sync(0xffffffffu, h1);
+            const int li = b0 ? __ffs(b0) - 1 : (b1 ? 31 + __ffs(b1) : 0);
+            if (lane == 0) ll_store(xpeak() + xp * 4 + aq, __int_as_float((int)aq * Tq + li), tag);
         }
         if (TR && cktr) cktr[6] = clock64();
         if (tid >= 128) return;
@@ -876,6 +938,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             finish(stage, t);
         }
     }
+    if (WIN && tid == 128 && aq == 0 && arow < B && A.peak) A.peak[(int64_t)arow * T + T - 1] = window_peak(T - 1, __float_as_int(misc_s[1]));
 }
 
 // ---- packing: TF [K][N] -> per-slice MMA A fragments [cs][warp][k-tile slot][lane][FL] ----
@@ -982,11 +1045,15 @@ void build_seg_table(SegDesc* sd, int64_t* total_floats) {
     *total_floats = off;
 }
 
-void build_ws_layout(int64_t* buf, int64_t* att, int64_t* total) {
+// word offsets of the exchange buffers, the attention exchange and the attention window's peak words; total = the end of
+// what each launch zeroes, where the per-stage trace of the TR instantiation starts (taco_decoder_trace_offset)
+void build_ws_layout(int64_t* buf, int64_t* att, int64_t* peak, int64_t* total) {
     int64_t o = 0;
     for (int b = 0; b < NBUF; ++b) { buf[b] = o; o += (int64_t)4 * buf_nkt(b) * 64; }
     *att = o;                                                    // [32 utterances][2][4] x (2 statistics + 256 context words)
     o += (int64_t)(NCTA / 4) * 2 * 4 * (2 + ENC);
+    *peak = o;                                                   // [32 utterances][2][4] peak words
+    o += (int64_t)(NCTA / 4) * 2 * 4;
     *total = o;
 }
 
@@ -1004,10 +1071,15 @@ int decoder_fwd_capacity(int* out) {
     TACO_CUDA(cudaGetDevice(&dev));
     TACO_CHECK(dev >= 0 && dev < MAX_DEVICES, "taco_decoder: device %d out of range", dev);
     if (cap[dev] == 0) {
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        int per_sm = 0, sms = 0;
-        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_kernel<false>, NTHR, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        int per_sm = 0, sms = 0, per_sm_w = 0;
+        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_kernel<false, false>, NTHR, 227 * 1024));
+        // the windowed kernel runs on the same grids: it has the same launch bounds and shared memory
+        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_w, decoder_kernel<false, true>, NTHR, 227 * 1024));
+        TACO_CHECK(per_sm_w == per_sm, "taco_decoder: windowed kernel occupancy %d != %d", per_sm_w, per_sm);
         TACO_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         cap[dev] = per_sm * sms > 0 ? per_sm * sms : -1;
     }
@@ -1035,9 +1107,15 @@ extern "C" size_t taco_decoder_packed_bytes(int r) {
 
 extern "C" size_t taco_decoder_workspace_bytes(int B, int Tx, int T, int r) {
     (void)B; (void)Tx; (void)r;
-    int64_t buf[NBUF], att, total;
-    build_ws_layout(buf, &att, &total);
+    int64_t buf[NBUF], att, peak, total;
+    build_ws_layout(buf, &att, &peak, &total);
     return (size_t)(total + trace_words(T)) * 8 + (size_t)INIT_FLOATS * 4;
+}
+
+extern "C" int64_t taco_decoder_trace_offset(void) {
+    int64_t buf[NBUF], att, peak, total;
+    build_ws_layout(buf, &att, &peak, &total);
+    return total;
 }
 
 extern "C" int taco_decoder_pack(const taco_decoder_weights* w, int r, float* packed, void* stream) {
@@ -1132,6 +1210,13 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
                "taco_decoder_fwd: workspace / packed must be 16-byte aligned");
     if (a->mode != TACO_DEC_INFER) TACO_CHECK(a->mel != nullptr, "taco_decoder_fwd: teacher/sched mode needs mel");
     if (a->mode == TACO_DEC_SCHED) TACO_CHECK(a->sample_mask != nullptr, "taco_decoder_fwd: sched mode needs sample_mask");
+    TACO_CHECK(a->win_back >= 0 && a->win_ahead >= 0, "taco_decoder_fwd: win_back=%d, win_ahead=%d: the attention window "
+               "bounds must be >= 0 (win_ahead = 0: no window)", a->win_back, a->win_ahead);
+    const bool win = a->win_ahead > 0;
+    TACO_CHECK(win || (a->win_back == 0 && a->peak == nullptr), "taco_decoder_fwd: win_ahead=0 (no window) with win_back=%d "
+               "and peak %s: a window needs win_ahead >= 1", a->win_back, a->peak ? "set" : "NULL");
+    TACO_CHECK(!win || a->mode == TACO_DEC_INFER, "taco_decoder_fwd: win_ahead=%d: the attention window applies to "
+               "free-running decoding (mode TACO_DEC_INFER) only, mode is %d", a->win_ahead, a->mode);
     TACO_CHECK((a->keep1 == nullptr) == (a->keep2 == nullptr), "taco_decoder_fwd: keep1/keep2 must both be set or both NULL");
     TACO_CHECK(a->row0 >= 0 && (a->row_stride == 0 ? a->row0 == 0 : a->row0 + a->B <= a->row_stride),
                "taco_decoder_fwd: rows [%d, %d) outside a row stride of %d", a->row0, a->row0 + a->B, a->row_stride);
@@ -1141,10 +1226,14 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     memset(&P, 0, sizeof(P));
     int64_t tot, ws_total;
     build_seg_table(P.seg, &tot);
-    build_ws_layout(P.buf, &P.att_off, &ws_total);
+    build_ws_layout(P.buf, &P.att_off, &P.peak_off, &ws_total);
     P.trace_off = ws_total;
     P.a = *a;
     if (P.a.row_stride == 0) P.a.row_stride = a->B;
+    if (win) {                          // a bound >= Tx allows every position already; p + ahead cannot overflow
+        P.a.win_back = a->win_back < a->Tx ? a->win_back : a->Tx;
+        P.a.win_ahead = a->win_ahead < a->Tx ? a->win_ahead : a->Tx;
+    }
     P.OUT = MF * a->r;
     P.NCY = (P.OUT + NS - 1) / NS;
     P.Tq = (a->Tx + 3) / 4;            // quarter width; the last quarter is ragged when Tx % 4 != 0
@@ -1250,8 +1339,9 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
         }
     }
     static const bool trace_build = getenv("TACO_TRACE") != nullptr;     // per-stage clock trace (scripts/dec_time.py)
-    if (trace_build && a->step_ns) TACO_CUDA(cudaLaunchKernelEx(&cfg, decoder_kernel<true>, P));
-    else                           TACO_CUDA(cudaLaunchKernelEx(&cfg, decoder_kernel<false>, P));
+    const bool trace = trace_build && a->step_ns;
+    if (win) TACO_CUDA(cudaLaunchKernelEx(&cfg, trace ? decoder_kernel<true, true> : decoder_kernel<false, true>, P));
+    else     TACO_CUDA(cudaLaunchKernelEx(&cfg, trace ? decoder_kernel<true, false> : decoder_kernel<false, false>, P));
     ++g_taco_launches;
     return 0;
 }

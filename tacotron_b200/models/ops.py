@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
+import numbers
 
 import torch
 
@@ -618,11 +619,36 @@ def decoder_plan(B, capacity, max_ctas=None):
     return [(b0, min(rows, B - b0), DEC_GROUP_CTAS * groups) for b0 in range(0, B, rows)]
 
 
-def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stream):
+INT32_MAX = 2 ** 31 - 1
+
+
+def attention_window(window):
+    """None (no window) or (back, ahead) -> None or a tuple of two ints with back >= 0 and ahead >= 1: the positions
+    step t of free-running decoding may attend are max(0, p(t-1) - back) .. p(t-1) + ahead, p(t-1) = the previous
+    step's attention peak (p(-1) = 0).  Both must fit taco_decoder_args' int32 fields.  Raises TacoError, before
+    anything is launched, for anything else."""
+    if window is None:
+        return None
+    try:
+        back, ahead = window
+    except (TypeError, ValueError):
+        raise L.TacoError(f"attention window {window!r}: expected None or (back, ahead)") from None
+    for name, v, lo in (("back", back, 0), ("ahead", ahead, 1)):
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+            raise L.TacoError(f"attention window {window!r}: {name} must be an integer, got {type(v).__name__}")
+        if v < lo:
+            raise L.TacoError(f"attention window {window!r}: {name} must be >= {lo}, got {v}")
+        if v > INT32_MAX:                     # the C ABI's int32 fields (any bound >= Tx already allows every position)
+            raise L.TacoError(f"attention window {window!r}: {name} must be <= {INT32_MAX}, got {v}")
+    return int(back), int(ahead)
+
+
+def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stream, window=None):
     """One taco_decoder_fwd per entry of `plan` over the full-batch tensors `t` (dict: packed, keys, values, text_length,
-    y, align, workspace, and mel, sample_mask, keep1, keep2, h_save, step_ns, h0, att0 or None).  [B]-major tensors are
-    passed from row b0; the [T][B]-major ones (sample_mask, keep1, keep2, h_save) and the initial states h0 [3][B][256],
-    att0 [B][256] whole, with row0 = b0 and row_stride = B."""
+    y, align, workspace, and mel, sample_mask, keep1, keep2, h_save, step_ns, h0, att0, peak or None).  [B]-major tensors
+    (peak [B][T] among them) are passed from row b0; the [T][B]-major ones (sample_mask, keep1, keep2, h_save) and the
+    initial states h0 [3][B][256], att0 [B][256] whole, with row0 = b0 and row_stride = B.  window: None or (back, ahead)
+    (attention_window), passed as given: taco_decoder_fwd checks it against the mode."""
     B = t["keys"].shape[0]
     Tx = t["keys"].shape[1]
     ptr = lambda x, b0=0: None if x is None else x[b0:].data_ptr()
@@ -642,13 +668,18 @@ def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stre
         a.step_ns = ptr(t.get("step_ns"))
         a.h0 = ptr(t.get("h0")); a.att0 = ptr(t.get("att0"))
         a.max_ctas = int(max_ctas or 0)
+        if window is not None:
+            a.win_back, a.win_ahead = window
+        a.peak = ptr(t.get("peak"), b0)
         L.check(lib.taco_decoder_fwd(C.byref(a), stream), "taco_decoder_fwd")
 
 
 def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sample_mask=None, drop_masks=None,
-                      dropout=0.5, scope=None, step_ns=None, max_ctas=None, h0=None, att0=None):
+                      dropout=0.5, scope=None, step_ns=None, max_ctas=None, h0=None, att0=None, window=None):
     """encoded [B,Tx,256], text_length int32 [B] -> (seq2seq_output [B,T,80r], alignments [B,T,Tx]).
     h0 [3,B,256] / att0 [B,256]: initial GRU states / attention vector (speaker-conditioned decoder), None = zero.
+    window: None, or (back, ahead) in free-running mode (attention_window): each step attends only near the previous
+    step's peak, and the result is (seq2seq_output, alignments, peaks int32 [B,T]) with each step's peak position.
     max_ctas caps the CTAs (SMs) the decoder kernel may occupy (None = all the device holds); the batch is decoded in as
     many launches of up to 8 x (max_ctas // 32) utterances as it needs (decoder_plan)."""
     from .. import kernels as K
@@ -656,6 +687,9 @@ def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sa
     rt = runtime(sc.store)
     B, Tx, D = encoded.shape
     assert D == 256
+    window = attention_window(window)
+    if window is not None and mode != L.DEC_INFER:
+        raise L.TacoError(f"attention window {window}: only free-running decoding (mode DEC_INFER) takes a window, mode is {mode}")
     lib = L.lib()
     plan = decoder_plan(B, K.decoder_capacity()[0], max_ctas)     # (raises before any launch for a budget below 32)
     out_w = 80 * r
@@ -706,5 +740,7 @@ def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sa
         assert k1.dtype == torch.uint8 and k1.shape == (T, B, 256) and k2.shape == (T, B, 128)
         assert k1.is_contiguous() and k2.is_contiguous()
         t["keep1"], t["keep2"] = k1, k2
-    decoder_fwd_launches(lib, plan, w, t, mode, T, r, ks, max_ctas, L.current_stream())
-    return y, align
+    if window is not None:
+        t["peak"] = rt.buf(sc.name("peak"), (B, T), torch.int32)
+    decoder_fwd_launches(lib, plan, w, t, mode, T, r, ks, max_ctas, L.current_stream(), window)
+    return (y, align) if window is None else (y, align, t["peak"])

@@ -61,6 +61,10 @@ class Config(object):
     # the text-speech diagonal outside which attention weight is penalised.  Training only; needs inputs['speech_steps'].
     guided_attention = 0.0
     guided_attention_g = 0.2
+    # attention window at synthesis (free-running decoding; training never uses it): None = off, or (back, ahead) with
+    # back >= 0, ahead >= 1: step t attends only positions p(t-1) - back .. p(t-1) + ahead around the previous step's
+    # attention peak p(t-1) (p(-1) = 0).  Off by default, as in the reference; each call also sets attention_peaks.
+    attention_window = None
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -81,6 +85,7 @@ class Tacotron(object):
         if max_ctas is not None:                  # a budget below one decoder row group fails here, before any launch
             from .. import kernels as K
             ops.decoder_budget(K.decoder_capacity()[0], max_ctas)
+        ops.attention_window(getattr(config, "attention_window", None))     # a malformed window fails here too
         self.config = config
         self.train = train
         self.device = torch.device(device)
@@ -90,6 +95,7 @@ class Tacotron(object):
         self.lr = config.init_lr
         self.global_step = 0
         self.seq2seq_output = self.output = self.alignments = self.loss = None
+        self.attention_peaks = None               # int32 [B, T] peak position of each decoder step (attention window on)
         self.guided_attention_loss = None
         self.step_ns = None
         self.section_wait = None
@@ -119,7 +125,8 @@ class Tacotron(object):
     def create_decoder(self, encoded, inputs, speaker_embed=None, train=True, T=None, dec_drop_masks=None,
                        sample_mask=None):
         """Returns a zero-argument callable that runs the whole decode (the BasicDecoder +
-        dynamic_decode pair of the reference) as one persistent kernel."""
+        dynamic_decode pair of the reference) as one persistent kernel: (seq2seq_output, alignments), and the step
+        peaks int32 [B, T] third when config.attention_window is set and train is False."""
         cfg = self.config
         if train:
             mel = inputs["mel"]
@@ -141,6 +148,7 @@ class Tacotron(object):
             T = cfg.max_decode_iter if T is None else T
             dec_drop_masks = None
             sample_mask = None
+        window = None if train else ops.attention_window(getattr(cfg, "attention_window", None))
         sc = ops.Scope(self.store, "dec")
         step_ns = self.step_ns
         if speaker_embed is not None and not getattr(cfg, "speaker_decoder", False):
@@ -153,7 +161,7 @@ class Tacotron(object):
             return ops.attention_decoder(encoded, inputs["text_length"], cfg.r, T, mode=mode, mel=mel,
                                          sample_mask=sample_mask, drop_masks=dec_drop_masks,
                                          dropout=cfg.audio_dropout_prob, scope=sc, step_ns=step_ns,
-                                         max_ctas=getattr(cfg, "max_ctas", None), h0=h0, att0=att0)
+                                         max_ctas=getattr(cfg, "max_ctas", None), h0=h0, att0=att0, window=window)
         return run
 
     # -- inference (tacotron.py:107-154) --------------------------------------------------------
@@ -227,7 +235,9 @@ class Tacotron(object):
         # attention decoder (:135-138)
         dec = self.create_decoder(encoded, inputs, self._decoder_speaker_embed(B), train, T=T, dec_drop_masks=dec_drop_masks,
                                   sample_mask=sample_mask)
-        seq2seq_output, self.alignments = dec()
+        res = dec()
+        seq2seq_output, self.alignments = res[:2]
+        self.attention_peaks = res[2] if len(res) > 2 else None
         self._mark("decoder")
         output = self._postnet(seq2seq_output, trace)
         self._mark("postnet")
@@ -235,7 +245,8 @@ class Tacotron(object):
 
     def _inference_graphed(self, inputs, T):
         T = self.config.max_decode_iter if T is None else T
-        key = (tuple(inputs["text"].shape), T, self.store.version, getattr(self.config, "max_ctas", None))
+        key = (tuple(inputs["text"].shape), T, self.store.version, getattr(self.config, "max_ctas", None),
+               ops.attention_window(getattr(self.config, "attention_window", None)))
         g = self._graphs.get(key) if hasattr(self, "_graphs") else None
         if g is None:
             if not hasattr(self, "_graphs"):
@@ -260,7 +271,9 @@ class Tacotron(object):
                 with torch.cuda.graph(gd, pool=pool):
                     dec = self.create_decoder(outs["encoded"], static, self._decoder_speaker_embed(static["text"].shape[0]),
                                               False, T=T)
-                    outs["y"], outs["align"] = dec()
+                    res = dec()
+                    outs["y"], outs["align"] = res[:2]
+                    outs["peak"] = res[2] if len(res) > 2 else None
                 gp = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(gp, pool=pool):
                     outs["out"] = self._postnet(outs["y"], None)
@@ -290,6 +303,7 @@ class Tacotron(object):
             cur.wait_event(waits["postnet"])
         graphs[2].replay(); self._mark("postnet")
         self.alignments = outs["align"]
+        self.attention_peaks = outs["peak"]
         self.last_graph_kernels = g[3]
         return outs["y"], outs["out"]
 

@@ -34,6 +34,16 @@ are joined with a pause set by the break between them and a 10 ms raised-cosine 
 driver writes ``<n>.wav``, ``<n>.txt`` (the whole line), ``<n>_chunks.txt`` (one chunk per line) and
 ``<n>_attention.npy`` (the block-diagonal stack of the chunk alignments), and with ``--summaries`` one audio and one
 image summary.  ``--trim-tail`` changes nothing here: long-form already trims.
+
+    python -m tacotron_b200.test -t nancy --attention-window          # back 2, ahead 5
+    python -m tacotron_b200.test -t nancy --attention-window 1,4
+
+``--attention-window [BACK,AHEAD]`` lets each decoder step attend only the characters from BACK behind to AHEAD ahead of
+the one the previous step attended most (the first step: the first character), so the alignment cannot jump ahead,
+fall far back or stick past the text.  It applies to every decode of the run, with or without ``--long-form``,
+``--trim-tail``, ``-s``, ``--max-ctas`` and ``--summaries``; the files written are the same ones.  The default 2,5 is
+close to the windows of common open Tacotron implementations and is a starting point only: no value has been tried on
+a trained model here.  Without the flag the decoder is the reference's.
 """
 from __future__ import annotations
 
@@ -48,7 +58,8 @@ import torch
 def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, trim_tail=False, long_form=False):
     """summary_dir: also write each prompt's audio and attention image as TensorBoard summaries there, at step 0
     (tacotron_b200/summary.py).  trim_tail: end each utterance where its speech ends; long_form: speak each line as one
-    clip, whatever its length (module docstring).  Returns one device waveform per prompt."""
+    clip, whatever its length (module docstring).  config.attention_window (None or (back, ahead)) applies to every
+    decode, plain and long-form.  Returns one device waveform per prompt."""
     from . import audio, checkpoint, data_input
     from .train import write_wav
     sr = 24000 if "blizzard" in config.data_path else 16000                              # test.py:15
@@ -207,6 +218,20 @@ def _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, 
     return waves
 
 
+def parse_attention_window(text):
+    """'BACK,AHEAD' -> (back, ahead) with back >= 0, ahead >= 1 (the --attention-window value)"""
+    parts = text.split(",")
+    try:
+        if len(parts) != 2:
+            raise ValueError
+        back, ahead = (int(v) for v in parts)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"{text!r}: expected BACK,AHEAD, two integers such as 2,5") from None
+    if back < 0 or ahead < 1:
+        raise argparse.ArgumentTypeError(f"{text!r}: BACK must be >= 0 and AHEAD >= 1")
+    return back, ahead
+
+
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", "--train-set", default="nancy")
@@ -219,6 +244,10 @@ def main(argv=None):
                              "decode the pieces as batches and join them")
     parser.add_argument("--max-ctas", type=int, default=None,
                         help="CTAs (SMs) the decoder kernels may occupy, at least 32 (default: all the device holds)")
+    parser.add_argument("--attention-window", type=parse_attention_window, nargs="?", const=(2, 5), default=None,
+                        metavar="BACK,AHEAD",
+                        help="attend only BACK characters behind to AHEAD ahead of the previous step's attention peak "
+                             "(a bare flag: 2,5, a starting point only)")
     args = parser.parse_args(argv)
     prompts = [p for p in sys.stdin.readlines() if len(p) > 0]                           # test.py:77-78
     from .models.tacotron import Config, Tacotron
@@ -226,6 +255,7 @@ def main(argv=None):
     config.data_path = "data/%s/" % args.train_set                                       # :83
     config.save_path = args.train_set + "/tacotron"                                      # :84
     config.max_ctas = args.max_ctas
+    config.attention_window = args.attention_window
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "test") if args.summaries else None      # test.py:33
     test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir, trim_tail=args.trim_tail,
