@@ -2,8 +2,9 @@
 
     TACO_TRACE=1 python scripts/dec_time.py [--precision fp32x3|tf32|fp32] [--window BACK,AHEAD]
 
-With TACO_TRACE set, the traced kernel instantiation also records per-slot and per-phase clocks of CTA 0; --window
-times the decoder with that attention window (Config.attention_window)."""
+With TACO_TRACE set, the traced kernel instantiation also records per-slot and per-phase clocks of CTA 0, and per-warp
+stage clocks of CTA 0 and CTA 48 (another row group) that split each slot into hop, barrier skew, epilogue and the rest;
+--window times the decoder with that attention window (Config.attention_window)."""
 import argparse, os, sys, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -59,3 +60,29 @@ if os.environ.get("TACO_TRACE"):
     if c[1, 3]:
         print("attention (cycles from slot start): q arrived+exp %d | bar1 %d | scores %d | bar2 %d | stats+bar3 %d | ctx partial+push %d | merged ctx stored %d"
               % tuple(int(statistics.median([int(c[st, i] - c[st, 3]) for st in range(3)])) for i in (0, 1, 2, 4, 5, 6, 7)))
+    # per-warp stage records [2 CTAs][3 steps][20 items][64]: [0,16) last on-chain word seen, [16,32) stage barrier
+    # reached, [32,48) barrier passed, [48,64) epilogue done (decoder.cu, trace_words)
+    wbase = int(L.lib().taco_decoder_trace_offset()) + 16 * T + 16 + 4 * 20 * 8 + 16
+    wr = ws[wbase: wbase + 2 * 3 * 20 * 64].reshape(2, 3, 20, 64)
+    epi = {"G1": 8, "C1": 2, "G2": 4, "C2": 2, "G3": 4, "C3": 2, "OQP": 8}     # warps with an epilogue role per stage
+    print("per-warp stage split [cycles, median of steps 10..12]: hop = previous stage's store (its last epilogue warp done)"
+          " -> last on-chain word seen by any warp | spread = first -> last warp's last word | skew = last word -> last warp at"
+          " the barrier | bar = -> warp 0 past it | epi0 / epiN = epilogue of warp 0 / of the last epilogue warp | slot = store"
+          " -> store")
+    for c, cta in enumerate((0, 48)):
+        if not (wr[c, :, :7, 48:64] > 0).all():
+            continue
+        print(f"  CTA {cta}:  stage    hop  spread   skew    bar   epi0   epiN   slot")
+        for i, nm in enumerate(names[:7]):
+            cols = []
+            for st in range(3):
+                r = wr[c, st, i].astype(np.int64)
+                arr, reach, passed, done = r[0:16], r[16:32], r[32:48], r[48:64]
+                ne = epi[nm]
+                store = done[:ne].max()
+                prev = wr[c, st, i - 1, 48:48 + epi[names[i - 1]]].astype(np.int64).max() if i > 0 else None
+                cols.append([arr.max() - prev if prev is not None else -1, arr.max() - arr.min(), reach.max() - arr.max(),
+                             passed[0] - reach.max(), done[0] - passed[0], done[ne - 1] - passed[ne - 1],
+                             store - prev if prev is not None else -1])
+            med = np.median(np.array(cols), axis=0).astype(int)
+            print(f"          {nm:5s} " + " ".join(f"{v:6d}" for v in med))

@@ -283,18 +283,31 @@ __device__ __forceinline__ void load_weights(float (&w)[N], uint32_t w1, uint32_
     }
 }
 // wait for the operand words v (loads already in flight) and multiply them into acc with weight fragments w (load_weights order)
+// TR: ck = thread 0's stage record (or NULL); wk = this warp's stamp of its last on-chain word (lane 0, or NULL)
 template <int FL, int MT, int NS_, bool TR, int N>
 __device__ __forceinline__ void multiply(float (&acc)[2][3][4], ulonglong2 (&v)[4], const float (&w)[N], const uint64_t* p0, int nkt, int widx,
-                                         int nw, int s0, uint32_t tag, long long* ck) {
+                                         int nw, int s0, uint32_t tag, long long* ck, long long* wk = nullptr) {
     if (TR && ck) ck[1] = clock64();
+    // three-slot G1 call (re-polling inside the loop below spills there): slot 1's word, stale when its load was issued
+    // before G1's off-chain halves, is requested again once, beside slot 0's first re-poll
+    if (NS_ == 3 && s0 <= 1 && widx + nw < nkt && !ll_ok(v[1], tag)) v[1] = ll_load2(p0 + (size_t)nw * 64);
 #pragma unroll
     for (int i = 0; i < NS_; ++i) {
         if (i >= s0 && widx + nw * i < nkt) {          // warp-uniform
-            ll_spin(v[i], p0 + (size_t)i * nw * 64, tag);
+            // two-slot calls: every poll of slot 0 also re-polls slot 1 while its word is stale, so that both are in flight
+            // together and slot 1's word is seen within the L2 round trip that finds slot 0's, not one round trip after it
+            // (its first load was issued before the producers published)
+            uint32_t spins = 0;
+            while (!ll_ok(v[i], tag)) {
+                if (++spins > (1u << 24)) __trap();
+                v[i] = ll_load2(p0 + (size_t)i * nw * 64);
+                if (NS_ == 2 && i == 0 && widx + nw < nkt && !ll_ok(v[1], tag)) v[1] = ll_load2(p0 + (size_t)nw * 64);
+            }
             uint32_t bh0, bl0, bh1, bl1;
             split_tf32(__uint_as_float((uint32_t)v[i].x), bh0, bl0);
             split_tf32(__uint_as_float((uint32_t)v[i].y), bh1, bl1);
             __syncwarp();                               // lanes arrive from divergent polling loops
+            if (TR && wk) *wk = clock64();
 #pragma unroll
             for (int mt = 0; mt < MT; ++mt) ktile_mma<FL>(acc[mt], bh0, bl0, bh1, bl1, &w[(mt * NS_ + i) * FL]);
         }
@@ -304,11 +317,11 @@ __device__ __forceinline__ void multiply(float (&acc)[2][3][4], ulonglong2 (&v)[
 template <int FL, int MT, int NS_, bool TR>
 __device__ __forceinline__ void consume(float (&acc)[2][3][4], ulonglong2 (&v)[4], const uint64_t* p0, int nkt, int widx, int nw, int s0,
                                         uint32_t tag, uint32_t w1, uint32_t w2, int wslot, const float* res_s, const float* packed,
-                                        int lane, long long* ck) {
+                                        int lane, long long* ck, long long* wk = nullptr) {
     float w[MT * NS_ * FL];
     __syncwarp();
     load_weights<FL, MT, NS_>(w, w1, w2, wslot, res_s, packed, lane);
-    multiply<FL, MT, NS_, TR>(acc, v, w, p0, nkt, widx, nw, s0, tag, ck);
+    multiply<FL, MT, NS_, TR>(acc, v, w, p0, nkt, widx, nw, s0, tag, ck, wk);
 }
 
 struct ItemRec { uint32_t flags, pre_base; int pre_tagd; uint32_t pre_w; uint32_t on_base; int on_tagd; uint32_t on_w1, on_w2; int on_nkt;
@@ -316,7 +329,8 @@ struct ItemRec { uint32_t flags, pre_base; int pre_tagd; uint32_t pre_w; uint32_
 // flags: kind | stage << 8 | has_pre << 16 | pre_skip0 << 17 | on_s0 << 20
 // s_*: the second off-chain operand of the G1 item, s(t-1), and its two weight tiles (SG_G1_S, SG_Z1_S)
 
-// TR: per-stage clock64 trace of CTA 0 (scripts/dec_time.py); the production instantiation has none of it.
+// TR: per-stage clock64 trace of CTA 0 (thread 0) and, per warp, of CTA 0 and CTA 48 (scripts/dec_time.py); the
+// production instantiation has none of it.
 // WIN: attention window (taco_decoder_args win_back / win_ahead, free-running decoding only): the scores outside
 // [p(t-1) - back, p(t-1) + ahead] are masked and each step's peak p(t) is found; without it the kernel is the plain one.
 template <bool TR, bool WIN>
@@ -469,6 +483,10 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     const bool tracer = (cta == 0 && tid == 0 && A.step_ns != nullptr);
     int64_t trace_i = 0;
     long long* cktr = nullptr;                          // per-item clock64 trace (CTA 0, thread 0, steps 10..13)
+    // per-warp stage records of CTA 0 and of CTA 48 (another row group), steps 10..12: [0, 16) last on-chain word seen,
+    // [16, 32) stage barrier reached, [32, 48) barrier passed, [48, 64) epilogue done; wtr = lane 0's word of its warp
+    const int trw = (TR && A.step_ns != nullptr) ? (cta == 0 ? 0 : cta == 48 ? 1 : -1) : -1;
+    long long* wtr = nullptr;
 
     // =========================================================================================================
     // finish a stage: per-warp partial tiles -> smem, cross-warp sum, epilogue (one thread per output)
@@ -771,8 +789,10 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
         if (stage == ST_G0) __syncthreads();
         store_partials(part, part_b, (stage == ST_OQP || stage == ST_G0) ? 2 : 1, full16);
         if (TR && cktr) cktr[4] = clock64();
+        if (TR && wtr) wtr[16] = clock64();
         __syncthreads();
         if (TR && cktr) cktr[5] = clock64();
+        if (TR && wtr) wtr[32] = clock64();
         const uint32_t tag = (uint32_t)t + 1;
         switch (stage) {
             case ST_G0: case ST_G1: case ST_G2:
@@ -834,6 +854,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             default: break;
         }
         if (TR && cktr) cktr[6] = clock64();
+        if (TR && wtr) wtr[48] = clock64();
         if (TR && tracer) ws[P.trace_off + (trace_i++)] = globaltimer_ns();
     };
 
@@ -873,6 +894,9 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             long long* ck = nullptr;
             if (TR && tracer && t >= 10 && t < 14) { ck = reinterpret_cast<long long*>(ws + P.trace_off + 16 * T + 16 + ((t - 10) * MAX_ITEMS + ii) * 8); ck[3] = clock64(); }
             cktr = ck;
+            wtr = (TR && trw >= 0 && lane == 0 && t >= 10 && t < 13)
+                ? reinterpret_cast<long long*>(ws + P.trace_off + 16 * T + 16 + 4 * MAX_ITEMS * 8 + 16 + ((trw * 3 + t - 10) * MAX_ITEMS + ii) * 64 + warp)
+                : nullptr;
             if (kind == IK_AP2) {
                 if (warp < 8) attention(t);
                 else if (t + 1 < T) prenet2(t + 1);
@@ -910,7 +934,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
                     load_weights<4, 2, 2>(wsx, rec.s_w1, rec.s_w2, warp * 2, res_s, packed, lane);
                     multiply<4, 2, 2, false>(acc, vp, wsx, psv, 32, warp, NWARP, 0, ptag, nullptr);
                 }
-                consume<4, 2, 3, TR>(acc, v, pon, (int)on_nkt, warp, NWARP, s0, otag, r1.z, r1.w, warp * 3, res_s, packed, lane, ck);
+                consume<4, 2, 3, TR>(acc, v, pon, (int)on_nkt, warp, NWARP, s0, otag, r1.z, r1.w, warp * 3, res_s, packed, lane, ck, wtr);
             } else {
                 if (has_pre && !pref) {
                     issue_loads<2>(vp, ppre, 32, warp, NWARP, 0);
@@ -919,12 +943,12 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
                 }
                 if (kind == IK_F4) {
                     if (has_pre) multiply<4, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
-                    consume<4, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
+                    consume<4, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck, wtr);
                 } else if (kind == IK_F2) {
                     if (has_pre) multiply<2, 1, 2, false>(acc, vp, wpre, ppre, 32, warp, NWARP, 0, ptag, nullptr);
-                    consume<2, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck);
+                    consume<2, 1, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, 0u, warp * 2, res_s, packed, lane, ck, wtr);
                 } else {
-                    consume<4, 2, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, r1.w, warp * 2, res_s, packed, lane, ck);
+                    consume<4, 2, 2, TR>(acc, v, pon, 32, warp, NWARP, 0, otag, r1.z, r1.w, warp * 2, res_s, packed, lane, ck, wtr);
                 }
             }
             pref = false;
@@ -1057,7 +1081,8 @@ void build_ws_layout(int64_t* buf, int64_t* att, int64_t* peak, int64_t* total) 
     *total = o;
 }
 
-inline int trace_words(int T) { return 16 * (T > 0 ? T : 0) + 16 + 4 * MAX_ITEMS * 8 + 16; }
+// [T] step stamps | thread 0's stage records [4 steps][MAX_ITEMS][8] | per-warp records [2 CTAs][3 steps][MAX_ITEMS][64]
+inline int trace_words(int T) { return 16 * (T > 0 ? T : 0) + 16 + 4 * MAX_ITEMS * 8 + 16 + 2 * 3 * MAX_ITEMS * 64; }
 // after the trace: the step-0 terms of an initial state, [32][512] floats each: init_z, init_zg (attention vector), then
 // [3][32][512] init_g (GRU states)
 constexpr int64_t INIT_ROWS = (int64_t)BPAD * 2 * U, INIT_FLOATS = 5 * INIT_ROWS;
