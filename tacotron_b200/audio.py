@@ -3,7 +3,7 @@
 it sits inside BASELINE config 5's end-to-end latency (test.py:64) and would dominate it on the CPU.
 
 Design: a batch of utterances stays on the device for all iterations.  The two transforms per iteration are the library's
-own shared-memory FFT kernels (csrc/audio.cu ``taco_rfft2048`` / ``taco_irfft2048``: radix-2 Stockham, one CTA per frame --
+own shared-memory FFT kernels (csrc/audio.cu ``taco_rfft2048`` / ``taco_irfft2048``: radix-4 Stockham, one CTA per frame --
 round 1 called cuFFT through ``torch.fft`` here); everything between them is four fused kernels of libtaco_b200.so:
 
     gl_init   reshape_frames(forward=False) + de-normalisation + exp + initial phase  ->  magnitude, first spectrum

@@ -209,10 +209,65 @@ __device__ __forceinline__ float rcp_fast(float x) {       // one MUFU.RCP (<= 1
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// e^{2x} with the argument clamped so that products of two such factors stay finite: exact for |x| <= 20.8
-// (tanh is saturated to the last bit far before that), graceful beyond
+// e^{2x} with the argument clamped to [-60, 60] (|x| > 20.79) so that products of two such factors stay finite.  Exact
+// while neither the key nor the query component is clamped.  Saturation is a property of k + q, not of k or q: past the
+// clamp e^{2k} e^{2q} no longer gives tanh(k + q) (k = 25, q = -24 would give tanh = 0 where tanh(1) = 0.76), so a step
+// whose keys or query reach the clamp is scored with tanhf_acc(k + q) instead (attention(), scores_direct).
 __device__ __forceinline__ float exp2x(float x) { return exp2f(fminf(fmaxf(x * 2.885390082f, -60.f), 60.f)); }
+__device__ __forceinline__ bool exp2x_clamps(float x) { return fabsf(x * 2.885390082f) > 60.f; }
+// bar.sync of `n` threads on barrier `id` that also returns whether any of them passed v = true
+__device__ __forceinline__ bool named_bar_or(int id, int n, bool v) {
+    int r;
+    asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.s32 q, %1, 0;\n\tbar.red.or.pred p, %2, %3, q;\n\tselp.s32 %0, 1, 0, p;\n\t}"
+                 : "=r"(r) : "r"((int)v), "r"(id), "r"(n) : "memory");
+    return r != 0;
+}
 __device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// Scores of one attention step in the direct form e_j = sum_d v_d tanhf_acc(k_jd + q_d), for a step where exp2x clamps,
+// over the same warp / lane / butterfly layout as the product form in attention().  keys = this utterance's [Tx][256]
+// keys, qw = its q(t) words in the exchange buffer (k-tile = 8 depths, pairs (p, p + 4) adjacent), positions jg = j0 + j
+// outside [lo, hi] are masked.  Out of line: the rare path costs the common one no registers.
+__device__ __noinline__ void scores_direct(float* e_s, const float* v_s, const float* keys, const uint64_t* qw, uint32_t tag,
+                                           int j0, int Tq, int Tx, int lo, int hi, int warp, int lane) {
+    float q[8], vv[8];
+#pragma unroll
+    for (int p = 0; p < 4; ++p) { const float2 qq = ll_wait2(qw + lane * 64 + 2 * p, tag); q[p] = qq.x; q[p + 4] = qq.y; }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) vv[i] = v_s[8 * lane + i];
+    for (int jb = 0; jb < Tq; jb += 32) {
+        float a4[4];
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const int j = jb + warp + 8 * jj, jg = j0 + j;
+            float a = 0.f;
+            if (j < Tq) {                               // keys past Tx are zero, as in e^{2 keys}
+#pragma unroll
+                for (int i = 0; i < 8; ++i)
+                    a = fmaf(vv[i], tanhf_acc((jg < Tx ? __ldg(keys + (int64_t)jg * 256 + 8 * lane + i) : 0.f) + q[i]), a);
+            }
+            a4[jj] = a;
+        }
+        float b2[2], b1;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const float send = (lane & 16) ? a4[k] : a4[k + 2];
+            const float keep = (lane & 16) ? a4[k + 2] : a4[k];
+            b2[k] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+        }
+        {
+            const float send = (lane & 8) ? b2[0] : b2[1];
+            const float keep = (lane & 8) ? b2[1] : b2[0];
+            b1 = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+        }
+        b1 += __shfl_xor_sync(0xffffffffu, b1, 4);
+        b1 += __shfl_xor_sync(0xffffffffu, b1, 2);
+        b1 += __shfl_xor_sync(0xffffffffu, b1, 1);
+        const int jj = ((lane >> 4) & 1) * 2 + ((lane >> 3) & 1);
+        const int j = jb + warp + 8 * jj;
+        if ((lane & 7) == 0 && j < Tq) e_s[j] = (j0 + j >= lo && j0 + j <= hi) ? b1 : -INFINITY;
+    }
+}
 
 // ---------------------------------------------------------------------------------------------
 // 3xTF32 tensor-core contraction pieces
@@ -343,7 +398,8 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     float* loc_s = part2_s + 512;                                 // h_loc[3][64] | u_loc[64] | z_loc[64] | cx_loc[64]
     float* bias_s = loc_s + 384;                                  // [NBR][16]
     float* att_s = bias_s + 256;                                  // eq[256] | v[256] | e[64] | p[64] | misc[64]
-                                                                  // (misc: V0 | p(t-1) of the window)
+                                                                  // (misc: V0 | p(t-1) of the window | a key of this
+                                                                  // CTA's slice reaches exp2x's clamp)
     ItemRec* itab = reinterpret_cast<ItemRec*>(att_s + 704);                 // [MAX_ITEMS] resolved stage records (20 x 12 words)
     uint32_t* otab = reinterpret_cast<uint32_t*>(itab + MAX_ITEMS);          // [NOUT] output word offsets of this CTA
     float* ek_s = smem + P.smem_kv_off;
@@ -446,6 +502,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
         }
     }
     // e^{2 keys} / values slice of (arow, aq) -> smem (padded rows), zero for utterances >= B and positions >= Tx
+    int kclamp = 0;                                     // a key of this slice reaches exp2x's clamp
     for (int i = tid; i < Tq * (ENC / 4); i += NTHR) {
         const int j = i / (ENC / 4), d4 = (i % (ENC / 4)) * 4;
         float4 kk = make_float4(0, 0, 0, 0), vv = kk;
@@ -454,19 +511,20 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             kk = __ldg(reinterpret_cast<const float4*>(A.keys + gi));
             vv = __ldg(reinterpret_cast<const float4*>(A.values + gi));
         }
+        kclamp |= exp2x_clamps(kk.x) | exp2x_clamps(kk.y) | exp2x_clamps(kk.z) | exp2x_clamps(kk.w);
         kk.x = exp2x(kk.x); kk.y = exp2x(kk.y); kk.z = exp2x(kk.z); kk.w = exp2x(kk.w);   // tanh(k+q) = 1 - 2/(e^{2k} e^{2q} + 1)
         *reinterpret_cast<float4*>(ek_s + j * KV_LD + d4) = kk;
         *reinterpret_cast<float4*>(vals_s + j * ENC + d4) = vv;
     }
     for (int i = tid; i < AU; i += NTHR) v_s[i] = __ldg(P.att_v + i);
     const int my_len = (arow < B) ? A.text_length[arow] : 0;
-    __syncthreads();
+    kclamp = __syncthreads_or(kclamp);
     if (warp == 0) {                                    // V0 = sum_d v_d  (e_j = V0 - 2 sum_d v_d / (E_jd + 1))
         float sv = 0.f;
         for (int i = lane; i < AU; i += 32) sv += v_s[i];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) sv += __shfl_xor_sync(0xffffffffu, sv, o);
-        if (lane == 0) misc_s[0] = sv;
+        if (lane == 0) { misc_s[0] = sv; misc_s[2] = kclamp ? 1.f : 0.f; }
     }
     __syncthreads();
 
@@ -566,20 +624,27 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             if (tid < 64) ll_store(ctx_out, 0.f, tag + 1);
             return;
         }
+        bool clamp = false;                             // q(t) or a key of this slice reaches exp2x's clamp
         if (tid < 128) {   // q(t) of this utterance -> e^{2q}
             const float2 qq = ll_wait2(ws + P.buf[B_Q] + (int64_t)(arow >> 3) * 2048 + (tid >> 2) * 64 + (arow & 7) * 8 + 2 * (tid & 3), tag);
             const int k0 = ((tid >> 2) << 3) + (tid & 3);        // physical pair (2p, 2p+1) = logical k0, k0+4
             eq_s[k0] = exp2x(qq.x);
             eq_s[k0 + 4] = exp2x(qq.y);
+            clamp = exp2x_clamps(qq.x) | exp2x_clamps(qq.y) | (tid == 0 && misc_s[2] != 0.f);
         } else if (WIN && tid == 128) {   // p(t-1), off the chain: its words are a step old, the poll runs beside q(t)'s
             const int pp = (t > 0) ? window_peak(t - 1, __float_as_int(misc_s[1])) : 0;
             misc_s[1] = __int_as_float(pp);
             if (t > 0 && aq == 0 && A.peak) A.peak[(int64_t)arow * T + t - 1] = pp;
         }
         if (TR && cktr) cktr[0] = clock64();
-        named_bar(1, 256);
+        clamp = named_bar_or(1, 256, clamp);            // (CTA-uniform; trained-like keys and queries never get there)
         if (TR && cktr) cktr[1] = clock64();
-        {   // scores: lane owns 8 consecutive depth indices (its e^{2q}, v slices stay in registers), warp w owns
+        if (clamp) scores_direct(e_s, v_s, A.keys + (int64_t)arow * Tx * ENC,
+                                 ws + P.buf[B_Q] + (int64_t)(arow >> 3) * 2048 + (arow & 7) * 8, tag, (int)aq * Tq, Tq, Tx,
+                                 WIN ? max(__float_as_int(misc_s[1]) - A.win_back, 0) : 0,
+                                 WIN ? min(__float_as_int(misc_s[1]) + A.win_ahead, min(my_len, Tx) - 1) : my_len - 1,
+                                 warp, lane);
+        else {   // scores: lane owns 8 consecutive depth indices (its e^{2q}, v slices stay in registers), warp w owns
             // positions j = w, w+8, ...; four positions are reduced over the warp with one transposing butterfly
             float eq[8], vv[8];
             {

@@ -232,7 +232,7 @@ def dec_inputs(Xin, sel, mel, y, sample_mask, r, sched):
     lo = (r - 1) * mf
     for t in range(T):
         x = mel[:, t, lo:lo + mf].clone()
-        s = torch.zeros(B, dtype=torch.bool)
+        s = torch.zeros(B, dtype=torch.bool, device=mel.device)
         if t > 0 and sched:
             s = sample_mask[t - 1].to(torch.bool)
             x = torch.where(s[:, None], y[:, t - 1, lo:lo + mf], x)
