@@ -48,8 +48,18 @@ template <class T> inline T __ldcs(const T* p) { return *p; }
 inline float __expf(float x) { return expf(x); }
 inline float __fdividef(float a, float b) { return a / b; }
 inline float __fdiv_rn(float a, float b) { return a / b; }
-inline float cospif(float x) { return (float)std::cos(M_PI * (double)x); }
-inline void sincospif(float x, float* s, float* c) { *s = (float)std::sin(M_PI * (double)x); *c = (float)std::cos(M_PI * (double)x); }
+// sin(pi x) and cos(pi x) as the device computes them: exact at multiples of 1/2 (sinpi(1) = 0, cospi(1/2) = 0, where
+// sin(M_PI) in double is 1.2e-16), otherwise the double value rounded once.  The argument is reduced exactly mod 2 first.
+inline void emu_sincospi(double x, double* s, double* c) {
+    const double r = std::fmod(x, 2.0);                                  // exact, in (-2, 2), sign of x
+    const double a = std::fabs(r);
+    if (a == 0.0 || a == 1.0) { *s = std::copysign(0.0, r); *c = a == 0.0 ? 1.0 : -1.0; return; }
+    if (a == 0.5 || a == 1.5) { *s = (a == 0.5) == (r > 0) ? 1.0 : -1.0; *c = 0.0; return; }
+    *s = std::sin(M_PI * r);
+    *c = std::cos(M_PI * r);
+}
+inline float cospif(float x) { double s, c; emu_sincospi(x, &s, &c); return (float)c; }
+inline void sincospif(float x, float* s, float* c) { double sd, cd; emu_sincospi(x, &sd, &cd); *s = (float)sd; *c = (float)cd; }
 inline uint32_t __float_as_uint(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
 inline float __uint_as_float(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
 inline int min(int a, int b) { return a < b ? a : b; }
