@@ -236,8 +236,21 @@ typedef struct taco_decoder_args {
                                     max(0, p(t-1) - win_back) <= j <= p(t-1) + win_ahead, j < N_b (the others are -inf
                                     before the softmax); p(t) = the lowest j of highest score.  win_back >= 0,
                                     win_ahead >= 1; bounds >= Tx - 1 allow every position and give the unwindowed bits */
-    int32_t*       peak;         /* [B][T] p(t) of each step (indexed like align), or NULL; needs the window          */
+    int32_t*       peak;         /* [B][T] p(t) of each step (indexed like align), or NULL; needs the window or the stop
+                                    rule (-1 at the steps a stopped row group did not decode)                            */
+    const int32_t* stop_at;      /* end-of-text stop rule (TACO_DEC_INFER only; NULL: off, the default).  [B] encoder   */
+    int32_t        stop_hold;    /* positions: row b ends after step t when p(t - stop_hold + 1), ..., p(t) are all >=
+                                    stop_at[b] (p as for peak, windowed or not), end_step[b] = t + 1 for the first such
+                                    t, or T.  stop_hold >= 1.  Each row group of 8 decodes D_g = min(T, max over its
+                                    rows of end_step + TACO_DECODER_STOP_LAG) steps (padding rows end at 0); at the
+                                    steps t >= D_g, y and align hold 0 and peak -1                                      */
+    int32_t*       end_step;     /* [B] out: end_step of each row (set with stop_at, NULL with it)                      */
 } taco_decoder_args;
+
+/* Steps a row group decodes past its last row's end_step under the stop rule: the row's end is known at the start of
+ * the next step's attention, every CTA of the group reads the group's ended rows one step later, and all of them leave
+ * at the top of the step after the next stage barrier (csrc/decoder.cu, DESIGN.md 3.4).                               */
+#define TACO_DECODER_STOP_LAG 3
 
 int taco_decoder_fwd(const taco_decoder_args* a, void* stream);
 /* co-resident CTAs of the forward (taco_decoder_fwd) and backward (taco_decoder_bwd) decoder kernels on the current

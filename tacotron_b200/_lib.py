@@ -73,7 +73,11 @@ class DecoderArgs(C.Structure):
         ("row0", C.c_int32), ("row_stride", C.c_int32), ("max_ctas", C.c_int32),
         ("h0", C.c_void_p), ("att0", C.c_void_p),
         ("win_back", C.c_int32), ("win_ahead", C.c_int32), ("peak", C.c_void_p),
+        ("stop_at", C.c_void_p), ("stop_hold", C.c_int32), ("end_step", C.c_void_p),
     ]
+
+
+DECODER_STOP_LAG = 3      # TACO_DECODER_STOP_LAG (include/taco_b200.h)
 
 
 class GemmDesc(C.Structure):

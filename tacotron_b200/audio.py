@@ -374,6 +374,19 @@ def speech_frames(spec, r, stft_mean=None, stft_std=None, top_db=TRIM_TOP_DB, K=
     return frames
 
 
+def stop_frames(end_step, r, T, frames=None):
+    """STFT frames to invert of each utterance of a decode the end-of-text stop rule ended (Tacotron.end_steps, T = the
+    steps the call returned) -> int32 [B] on end_step's device, without a host synchronisation: min(4r ceil(end_step[b] /
+    4), 4r (T // 4)), at least the 5 frames invert_speech needs, and at most frames[b] when frames (e.g. speech_frames
+    with --trim-tail) is given."""
+    n = 4 * r * (T // 4)
+    lo = -(-5 // (4 * r)) * 4 * r
+    f = ((end_step.to(torch.int64) + 3) // 4 * (4 * r)).clamp(min=min(lo, n), max=n)
+    if frames is not None:
+        f = torch.minimum(f, frames.to(torch.int64))
+    return f.to(torch.int32)
+
+
 def invert_speech(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, generator=None):
     """invert_spectrogram on the first frames[b] STFT frames of each utterance only (frames: speech_frames or the
     caller's, a multiple of 4r in [5, 4r*(T//4)] each) -> list of B 1-D waveforms of hop*(frames[b]-1) samples.  The kept

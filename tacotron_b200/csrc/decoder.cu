@@ -57,6 +57,10 @@
 //     four (lowest quarter holding the utterance's max) beside the q(t+1) polls, so no new exchange sits on the chain
 //     (the windowed step still measures ~0.3 us longer, DESIGN.md 3.4).  The off instantiation is the plain kernel,
 //     instruction for instruction.
+//   * end-of-text stop rule (opt-in, free-running decoding; decoder_kernel<.., WIN = true, STOP = true>): thread 128 of
+//     each utterance's quarter-0 CTA counts the run of peaks >= stop_at and publishes one tagged status word per step;
+//     a step later, lanes 0-7 of warp 5 of every CTA of the row group read the group's 8 words beside the q polls, and
+//     all 32 CTAs leave at the top of the same step once every row has ended (TACO_DECODER_STOP_LAG, DESIGN.md 3.4).
 //
 // Unchanged from v3: grid = 32 co-resident CTAs per row group of 8 utterances (128 = 4 row groups when the device holds
 // them), CTA (rg, cs) owns utterance rows 8rg..8rg+7 and the
@@ -132,6 +136,7 @@ struct DecParams {
     int64_t buf[NBUF];           // word offsets of the exchange buffers
     int64_t att_off;             // word offset of the attention exchange region
     int64_t peak_off;            // word offset of the attention window's peak words
+    int64_t stop_off;            // word offset of the stop rule's status words (after the initial-state terms)
     int64_t trace_off;
     taco_decoder_args a;
     const float *gru_bg[3], *gru_bc[3], *out_b, *pre_b1, *pre_b2, *att_v;
@@ -388,8 +393,11 @@ struct ItemRec { uint32_t flags, pre_base; int pre_tagd; uint32_t pre_w; uint32_
 // production instantiation has none of it.
 // WIN: attention window (taco_decoder_args win_back / win_ahead, free-running decoding only): the scores outside
 // [p(t-1) - back, p(t-1) + ahead] are masked and each step's peak p(t) is found; without it the kernel is the plain one.
-template <bool TR, bool WIN>
+// STOP (implies WIN): the end-of-text stop rule (taco_decoder_args stop_at / stop_hold / end_step): each row group
+// leaves the step loop once every row of it has ended (see stop_poll).
+template <bool TR, bool WIN, bool STOP>
 __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant__ DecParams P) {
+    static_assert(WIN || !STOP, "the stop rule needs the windowed kernel's peaks");
     extern __shared__ __align__(16) float smem[];
     // smem map (floats): [0,16) reserved | part 6400 | part2 512 | loc 384 | bias 256 | att 704 | itab 256 | kv | weights
     float* part_s = smem + 16;                                    // [3 buffers][16 warps][PPITCH]: two alternate, the third is the
@@ -399,7 +407,9 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     float* bias_s = loc_s + 384;                                  // [NBR][16]
     float* att_s = bias_s + 256;                                  // eq[256] | v[256] | e[64] | p[64] | misc[64]
                                                                   // (misc: V0 | p(t-1) of the window | a key of this
-                                                                  // CTA's slice reaches exp2x's clamp)
+                                                                  // CTA's slice reaches exp2x's clamp | stop rule: run
+                                                                  // of peaks >= stop_at | end step (0: running) |
+                                                                  // step to leave at | stop_at)
     ItemRec* itab = reinterpret_cast<ItemRec*>(att_s + 704);                 // [MAX_ITEMS] resolved stage records (20 x 12 words)
     uint32_t* otab = reinterpret_cast<uint32_t*>(itab + MAX_ITEMS);          // [NOUT] output word offsets of this CTA
     float* ek_s = smem + P.smem_kv_off;
@@ -525,6 +535,11 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) sv += __shfl_xor_sync(0xffffffffu, sv, o);
         if (lane == 0) { misc_s[0] = sv; misc_s[2] = kclamp ? 1.f : 0.f; }
+        if (STOP && lane == 0) {                        // stop rule state (misc_i[3..6])
+            int* mi = reinterpret_cast<int*>(misc_s);
+            mi[3] = 0; mi[4] = 0; mi[5] = T;
+            mi[6] = arow < B ? A.stop_at[arow] : 0;
+        }
     }
     __syncthreads();
 
@@ -615,11 +630,44 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
         return p;
     };
 
+    // ---- stop rule (STOP instantiation): thread 128 of the quarter-0 CTA of each
+    //      utterance counts the run of peaks >= stop_at and publishes one status word per step, {end step or 0, tag};
+    //      thread 160 of every CTA of the row group reads its group's words a step later and sets the step all of them
+    //      leave at.  Every CTA reads the same published words, so every CTA picks the same step ----
+    //      Status words: [32 utterances][2 parity] {end step or 0 = running, tag t + 1}.  misc_i[3] = the run of peaks
+    //      >= stop_at, [4] = the end step, [5] = the step to leave at, [6] = stop_at ----
+    auto xstop = [&](int row, int ts) { return ws + P.stop_off + (int64_t)row * 2 + (ts & 1); };
+    auto stop_publish = [&](int t, int pp) {            // at step t, with pp = p(t - 1)
+        int* mi = reinterpret_cast<int*>(misc_s);
+        int end = mi[4];
+        if (t > 0 && end == 0) {
+            const int run = pp >= mi[6] ? mi[3] + 1 : 0;
+            mi[3] = run;
+            if (run >= A.stop_hold) { end = t; mi[4] = end; }
+        }
+        ll_store(xstop(arow, t), __int_as_float(end), (uint32_t)t + 1);
+    };
+    // at step t >= 1 on lanes 0..7 of warp 5 (one row each): the words of step t - 1, a step old.  Once every row has
+    // ended (padding rows have) the CTA leaves at the top of step t + 2: G1(t + 1)'s __syncthreads lies between this
+    // store and every thread's read
+    auto stop_poll = [&](int t) {
+        const int i = tid - 160;
+        bool ended = true;
+        if (row0 + i < B) {
+            uint64_t w = ll_load1(xstop(row0 + i, t - 1));
+            ended = __float_as_int(ll_spin1(w, xstop(row0 + i, t - 1), (uint32_t)t)) != 0;
+        }
+        volatile int* mi = reinterpret_cast<volatile int*>(misc_s);
+        if (__all_sync(0xffu, ended) && i == 0 && mi[5] > t + 2) mi[5] = t + 2;
+    };
+
     // ---- attention of step t on warps 0..7 (256 threads): scores, partial softmax / context, merge of the quarters ----
     auto attention = [&](int t) {
         const uint32_t tag = (uint32_t)t + 1;
         const int xp = t & 1;
         uint64_t* ctx_out = ws + P.buf[B_CP] + (int64_t)(arow >> 3) * 48 * 64 + (8 * (int)aq + ((tid & 63) >> 3)) * 64 + (arow & 7) * 8 + perm8(tid & 7);
+        if (STOP && tid >= 160 && tid < 160 + RPG && t > 0) stop_poll(t);   // (idle during the q(t) polls;
+                                                                                          // also in padding CTAs)
         if (arow >= B) {                                // padding utterance: publish a zero context (consumers poll every row)
             if (tid < 64) ll_store(ctx_out, 0.f, tag + 1);
             return;
@@ -635,6 +683,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             const int pp = (t > 0) ? window_peak(t - 1, __float_as_int(misc_s[1])) : 0;
             misc_s[1] = __int_as_float(pp);
             if (t > 0 && aq == 0 && A.peak) A.peak[(int64_t)arow * T + t - 1] = pp;
+            if (STOP && aq == 0) stop_publish(t, pp);
         }
         if (TR && cktr) cktr[0] = clock64();
         clamp = named_bar_or(1, 256, clamp);            // (CTA-uniform; trained-like keys and queries never get there)
@@ -950,6 +999,7 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
     uint4 nr0, nr1; uint32_t nnkt;
     ld_rec(0, nr0, nr1, nnkt);
     for (int t = 0; t < T; ++t) {
+        if (STOP && t >= reinterpret_cast<volatile int*>(misc_s)[5]) break;   // CTA-uniform and group-uniform
         if (tracer) A.step_ns[t] = globaltimer_ns();
         for (int ii = 0; ii < n_items; ++ii) {
             // r0 = flags, pre_base, pre_tagd, pre_w;  r1 = on_base, on_tagd, on_w1, on_w2 -- fetched one stage ahead
@@ -1027,7 +1077,30 @@ __global__ void __launch_bounds__(NTHR, 1) decoder_kernel(const __grid_constant_
             finish(stage, t);
         }
     }
-    if (WIN && tid == 128 && aq == 0 && arow < B && A.peak) A.peak[(int64_t)arow * T + T - 1] = window_peak(T - 1, __float_as_int(misc_s[1]));
+    // steps decoded: T, or the step the stop rule left at (a later write of misc_i[5] by stop_poll can only be >= T)
+    const int t_end = STOP ? min(reinterpret_cast<volatile int*>(misc_s)[5], T) : T;
+    if (WIN && tid == 128 && aq == 0 && arow < B && A.peak)
+        A.peak[(int64_t)arow * T + t_end - 1] = window_peak(t_end - 1, __float_as_int(misc_s[1]));
+    if (STOP) {
+        if (tid == 128 && aq == 0 && arow < B) {
+            const int end = reinterpret_cast<int*>(misc_s)[4];
+            A.end_step[arow] = end > 0 ? end : T;
+        }
+        // the steps the group did not decode: y and align 0, peak -1 (this CTA's columns / quarter / row)
+        const int nt = T - t_end;
+        for (int i = tid; i < nt * RPG * NCY; i += NTHR) {
+            const int tt = t_end + i / (RPG * NCY), br = (i / NCY) % RPG, wc = i % NCY, col = cs * NCY + wc;
+            if (row0 + br < B && col < OUT) A.y[((int64_t)(row0 + br) * T + tt) * OUT + col] = 0.f;
+        }
+        if (arow < B) {
+            for (int i = tid; i < nt * Tq; i += NTHR) {
+                const int tt = t_end + i / Tq, j = (int)aq * Tq + i % Tq;
+                if (j < Tx) A.align[((int64_t)arow * T + tt) * Tx + j] = 0.f;
+            }
+            if (aq == 0 && A.peak)
+                for (int i = tid; i < nt; i += NTHR) A.peak[(int64_t)arow * T + t_end + i] = -1;
+        }
+    }
 }
 
 // ---- packing: TF [K][N] -> per-slice MMA A fragments [cs][warp][k-tile slot][lane][FL] ----
@@ -1151,6 +1224,9 @@ inline int trace_words(int T) { return 16 * (T > 0 ? T : 0) + 16 + 4 * MAX_ITEMS
 // after the trace: the step-0 terms of an initial state, [32][512] floats each: init_z, init_zg (attention vector), then
 // [3][32][512] init_g (GRU states)
 constexpr int64_t INIT_ROWS = (int64_t)BPAD * 2 * U, INIT_FLOATS = 5 * INIT_ROWS;
+// after those: the stop rule's status words, [32 utterances][2 parity] (zeroed by the launches that use them)
+constexpr int64_t STOP_WORDS = (int64_t)(NCTA / 4) * 2;
+inline int64_t stop_words_offset(int64_t ws_total, int T) { return ws_total + trace_words(T) + INIT_FLOATS / 2; }
 
 // co-resident CTAs of the forward kernel on the current device (computed once per device; a MIG instance or an H100 PCIe
 // has fewer SMs than the 132 of an H100 SXM).  Also opts the kernel into the full 227 KB of shared memory on that device.
@@ -1161,15 +1237,19 @@ int decoder_fwd_capacity(int* out) {
     TACO_CUDA(cudaGetDevice(&dev));
     TACO_CHECK(dev >= 0 && dev < MAX_DEVICES, "taco_decoder: device %d out of range", dev);
     if (cap[dev] == 0) {
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        int per_sm = 0, sms = 0, per_sm_w = 0;
-        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_kernel<false, false>, NTHR, 227 * 1024));
-        // the windowed kernel runs on the same grids: it has the same launch bounds and shared memory
-        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_w, decoder_kernel<false, true>, NTHR, 227 * 1024));
-        TACO_CHECK(per_sm_w == per_sm, "taco_decoder: windowed kernel occupancy %d != %d", per_sm_w, per_sm);
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        TACO_CUDA(cudaFuncSetAttribute(decoder_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        int per_sm = 0, sms = 0, per_sm_w = 0, per_sm_s = 0;
+        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decoder_kernel<false, false, false>, NTHR, 227 * 1024));
+        // the windowed and stopping kernels run on the same grids: they have the same launch bounds and shared memory
+        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_w, decoder_kernel<false, true, false>, NTHR, 227 * 1024));
+        TACO_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_s, decoder_kernel<false, true, true>, NTHR, 227 * 1024));
+        TACO_CHECK(per_sm_w == per_sm && per_sm_s == per_sm, "taco_decoder: windowed / stopping kernel occupancy %d / %d != %d",
+                   per_sm_w, per_sm_s, per_sm);
         TACO_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         cap[dev] = per_sm * sms > 0 ? per_sm * sms : -1;
     }
@@ -1199,7 +1279,7 @@ extern "C" size_t taco_decoder_workspace_bytes(int B, int Tx, int T, int r) {
     (void)B; (void)Tx; (void)r;
     int64_t buf[NBUF], att, peak, total;
     build_ws_layout(buf, &att, &peak, &total);
-    return (size_t)(total + trace_words(T)) * 8 + (size_t)INIT_FLOATS * 4;
+    return (size_t)(stop_words_offset(total, T) + STOP_WORDS) * 8;
 }
 
 extern "C" int64_t taco_decoder_trace_offset(void) {
@@ -1303,10 +1383,19 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     TACO_CHECK(a->win_back >= 0 && a->win_ahead >= 0, "taco_decoder_fwd: win_back=%d, win_ahead=%d: the attention window "
                "bounds must be >= 0 (win_ahead = 0: no window)", a->win_back, a->win_ahead);
     const bool win = a->win_ahead > 0;
-    TACO_CHECK(win || (a->win_back == 0 && a->peak == nullptr), "taco_decoder_fwd: win_ahead=0 (no window) with win_back=%d "
-               "and peak %s: a window needs win_ahead >= 1", a->win_back, a->peak ? "set" : "NULL");
+    TACO_CHECK(win || (a->win_back == 0 && (a->peak == nullptr || a->stop_at != nullptr)), "taco_decoder_fwd: win_ahead=0 "
+               "(no window) with win_back=%d and peak %s: a window needs win_ahead >= 1 (peak: or the stop rule)",
+               a->win_back, a->peak ? "set" : "NULL");
     TACO_CHECK(!win || a->mode == TACO_DEC_INFER, "taco_decoder_fwd: win_ahead=%d: the attention window applies to "
                "free-running decoding (mode TACO_DEC_INFER) only, mode is %d", a->win_ahead, a->mode);
+    const bool stop = a->stop_at != nullptr;
+    TACO_CHECK(stop == (a->end_step != nullptr), "taco_decoder_fwd: stop_at %s with end_step %s: the stop rule needs both "
+               "(or neither)", a->stop_at ? "set" : "NULL", a->end_step ? "set" : "NULL");
+    TACO_CHECK(stop || a->stop_hold == 0, "taco_decoder_fwd: stop_hold=%d without stop_at", a->stop_hold);
+    TACO_CHECK(!stop || a->stop_hold >= 1, "taco_decoder_fwd: stop_hold=%d: the stop rule needs a hold of >= 1 step",
+               a->stop_hold);
+    TACO_CHECK(!stop || a->mode == TACO_DEC_INFER, "taco_decoder_fwd: the stop rule applies to free-running decoding "
+               "(mode TACO_DEC_INFER) only, mode is %d", a->mode);
     TACO_CHECK((a->keep1 == nullptr) == (a->keep2 == nullptr), "taco_decoder_fwd: keep1/keep2 must both be set or both NULL");
     TACO_CHECK(a->row0 >= 0 && (a->row_stride == 0 ? a->row0 == 0 : a->row0 + a->B <= a->row_stride),
                "taco_decoder_fwd: rows [%d, %d) outside a row stride of %d", a->row0, a->row0 + a->B, a->row_stride);
@@ -1323,7 +1412,11 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     if (win) {                          // a bound >= Tx allows every position already; p + ahead cannot overflow
         P.a.win_back = a->win_back < a->Tx ? a->win_back : a->Tx;
         P.a.win_ahead = a->win_ahead < a->Tx ? a->win_ahead : a->Tx;
+    } else if (stop) {                  // the stop rule needs the peaks: the windowed kernel, with bounds that cover every
+        P.a.win_back = a->Tx;           // position (the unwindowed bits)
+        P.a.win_ahead = a->Tx;
     }
+    P.stop_off = stop_words_offset(ws_total, a->T);
     P.OUT = MF * a->r;
     P.NCY = (P.OUT + NS - 1) / NS;
     P.Tq = (a->Tx + 3) / 4;            // quarter width; the last quarter is ragged when Tx % 4 != 0
@@ -1395,6 +1488,7 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     coop.val.cooperative = 1;
     cfg.attrs = &coop; cfg.numAttrs = 1;
     TACO_CUDA(cudaMemsetAsync(a->workspace, 0, (size_t)ws_total * 8, st));
+    if (stop) TACO_CUDA(cudaMemsetAsync(reinterpret_cast<uint64_t*>(a->workspace) + P.stop_off, 0, STOP_WORDS * 8, st));
     // initial state (speaker-conditioned decoder): the kernel skips the h(t-1) and attention products at t = 0, so their
     // step-0 values are formed here, per row of this launch, and added by the G1 and G epilogues of step 0 (the C stage
     // sees h0 through r * h and the state update): with iz = att0 . W_in[128:], init_z = [iz . Wc1_x | iz] and
@@ -1430,8 +1524,9 @@ extern "C" int taco_decoder_fwd(const taco_decoder_args* a, void* stream) {
     }
     static const bool trace_build = getenv("TACO_TRACE") != nullptr;     // per-stage clock trace (scripts/dec_time.py)
     const bool trace = trace_build && a->step_ns;
-    if (win) TACO_CUDA(cudaLaunchKernelEx(&cfg, trace ? decoder_kernel<true, true> : decoder_kernel<false, true>, P));
-    else     TACO_CUDA(cudaLaunchKernelEx(&cfg, trace ? decoder_kernel<true, false> : decoder_kernel<false, false>, P));
+    if (stop)     TACO_CUDA(cudaLaunchKernelEx(&cfg, trace ? decoder_kernel<true, true, true> : decoder_kernel<false, true, true>, P));
+    else if (win) TACO_CUDA(cudaLaunchKernelEx(&cfg, trace ? decoder_kernel<true, true, false> : decoder_kernel<false, true, false>, P));
+    else          TACO_CUDA(cudaLaunchKernelEx(&cfg, trace ? decoder_kernel<true, false, false> : decoder_kernel<false, false, false>, P));
     ++g_taco_launches;
     return 0;
 }

@@ -643,12 +643,61 @@ def attention_window(window):
     return int(back), int(ahead)
 
 
-def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stream, window=None):
+def stop_rule_hold(hold):
+    """None (no stop rule) or hold -> None or an int >= 1: the decoder steps in a row whose attention peaks must all lie
+    at or past the last real character before a row ends (the end-of-text stop rule of free-running decoding).  It must
+    fit taco_decoder_args' int32 field.  Raises TacoError, before anything is launched, for anything else."""
+    if hold is None:
+        return None
+    if isinstance(hold, bool) or not isinstance(hold, numbers.Integral):
+        raise L.TacoError(f"stop rule hold {hold!r}: expected None or an integer >= 1, got {type(hold).__name__}")
+    if not 1 <= hold <= INT32_MAX:
+        raise L.TacoError(f"stop rule hold {hold!r}: must be in [1, {INT32_MAX}]")
+    return int(hold)
+
+
+def stop_positions(text, text_length):
+    """stop_at int32 [B] on text's device, without a host synchronisation: the position of each row's last real
+    character, max(min(n_b, N_b, Tx) - 1, 0), with n_b = the non-zero ids of text row b (id 0 is <pad>) and N_b =
+    text_length[b].  N_b alone is not it: load_prompts counts the raw line, newline included, in text_length while
+    dropping out-of-vocabulary characters from the ids, so position N_b - 1 is usually padding."""
+    B, Tx = text.shape
+    n = (text != 0).sum(dim=1)
+    last = torch.minimum(torch.minimum(n, text_length.to(n.dtype)), torch.full_like(n, Tx)) - 1
+    return last.clamp_(min=0).to(torch.int32)
+
+
+def stop_rule_end_steps(peaks, stop_at, hold):
+    """The stop rule on a host array of peaks [B, T] (each step's attention peak p(t)): end_step [B] int64 = t + 1 for
+    the first t with p(t - hold + 1), ..., p(t) all >= stop_at[b], or T.  The kernel applies the same rule to its own
+    peaks as it decodes."""
+    import numpy as np
+    p = np.asarray(peaks)
+    B, T = p.shape
+    at = np.asarray(stop_at).reshape(B, 1)
+    end = np.full(B, T, dtype=np.int64)
+    run = np.zeros(B, dtype=np.int64)
+    for t in range(T):
+        run = np.where(p[:, t] >= at[:, 0], run + 1, 0)
+        hit = (run >= hold) & (end == T)
+        end[hit] = t + 1
+    return end
+
+
+def stopped_steps(end_step, T):
+    """decoder steps Tacotron.inference keeps from a stopped decode of T steps: T' = min(T, 4 ceil(max_b end_step / 4)),
+    whole blocks of 4 steps as reshape_frames needs.  Reads end_step to the host (one synchronisation)."""
+    e = int(end_step.max()) if torch.is_tensor(end_step) else int(max(end_step))
+    return min(int(T), 4 * ((e + 3) // 4))
+
+
+def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stream, window=None, hold=None):
     """One taco_decoder_fwd per entry of `plan` over the full-batch tensors `t` (dict: packed, keys, values, text_length,
     y, align, workspace, and mel, sample_mask, keep1, keep2, h_save, step_ns, h0, att0, peak or None).  [B]-major tensors
     (peak [B][T] among them) are passed from row b0; the [T][B]-major ones (sample_mask, keep1, keep2, h_save) and the
     initial states h0 [3][B][256], att0 [B][256] whole, with row0 = b0 and row_stride = B.  window: None or (back, ahead)
-    (attention_window), passed as given: taco_decoder_fwd checks it against the mode."""
+    (attention_window), passed as given: taco_decoder_fwd checks it against the mode.  hold: None or the stop rule's hold
+    (stop_rule_hold), with t['stop_at'] and t['end_step'] int32 [B], passed from row b0 like peak."""
     B = t["keys"].shape[0]
     Tx = t["keys"].shape[1]
     ptr = lambda x, b0=0: None if x is None else x[b0:].data_ptr()
@@ -671,25 +720,45 @@ def decoder_fwd_launches(lib, plan, w, t, mode, T, r, keep_scale, max_ctas, stre
         if window is not None:
             a.win_back, a.win_ahead = window
         a.peak = ptr(t.get("peak"), b0)
+        a.stop_at = ptr(t.get("stop_at"), b0); a.end_step = ptr(t.get("end_step"), b0)
+        if hold is not None:
+            a.stop_hold = hold
         L.check(lib.taco_decoder_fwd(C.byref(a), stream), "taco_decoder_fwd")
 
 
 def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sample_mask=None, drop_masks=None,
-                      dropout=0.5, scope=None, step_ns=None, max_ctas=None, h0=None, att0=None, window=None):
+                      dropout=0.5, scope=None, step_ns=None, max_ctas=None, h0=None, att0=None, window=None,
+                      stop_hold=None, stop_at=None):
     """encoded [B,Tx,256], text_length int32 [B] -> (seq2seq_output [B,T,80r], alignments [B,T,Tx]).
     h0 [3,B,256] / att0 [B,256]: initial GRU states / attention vector (speaker-conditioned decoder), None = zero.
     window: None, or (back, ahead) in free-running mode (attention_window): each step attends only near the previous
     step's peak, and the result is (seq2seq_output, alignments, peaks int32 [B,T]) with each step's peak position.
+    stop_hold, stop_at: None, or the end-of-text stop rule in free-running mode, both set: hold (stop_rule_hold) >= 1 and
+    stop_at int32 [B] (stop_positions).  Row b ends after step t when p(t - hold + 1), ..., p(t) >= stop_at[b];
+    end_step[b] = t + 1, or T.  Each row group of 8 stops decoding within _lib.DECODER_STOP_LAG steps of its last row's
+    end; the steps it did not decode hold 0 in y and alignments and -1 in the peaks.  The result is then
+    (seq2seq_output, alignments, peaks, end_step int32 [B]), on the device (nothing is read to the host).
     max_ctas caps the CTAs (SMs) the decoder kernel may occupy (None = all the device holds); the batch is decoded in as
     many launches of up to 8 x (max_ctas // 32) utterances as it needs (decoder_plan)."""
     from .. import kernels as K
-    sc = scope or current_scope()
-    rt = runtime(sc.store)
     B, Tx, D = encoded.shape
     assert D == 256
     window = attention_window(window)
     if window is not None and mode != L.DEC_INFER:
         raise L.TacoError(f"attention window {window}: only free-running decoding (mode DEC_INFER) takes a window, mode is {mode}")
+    hold = stop_rule_hold(stop_hold)
+    if (hold is None) != (stop_at is None):
+        raise L.TacoError(f"stop rule: stop_hold={stop_hold!r} and stop_at {'set' if stop_at is not None else 'None'}: "
+                          f"give both or neither")
+    if hold is not None:
+        if mode != L.DEC_INFER:
+            raise L.TacoError(f"stop rule: only free-running decoding (mode DEC_INFER) stops at the end of the text, mode is {mode}")
+        if not (stop_at.dtype == torch.int32 and stop_at.is_contiguous() and tuple(stop_at.shape) == (B,)
+                and stop_at.device == encoded.device):
+            raise L.TacoError(f"stop rule: stop_at must be a contiguous int32 tensor of shape [{B}] on {encoded.device}, got "
+                              f"{stop_at.dtype} {stop_at.device} {tuple(stop_at.shape)}")
+    sc = scope or current_scope()
+    rt = runtime(sc.store)
     lib = L.lib()
     plan = decoder_plan(B, K.decoder_capacity()[0], max_ctas)     # (raises before any launch for a budget below 32)
     out_w = 80 * r
@@ -740,7 +809,12 @@ def attention_decoder(encoded, text_length, r, T, mode=L.DEC_INFER, mel=None, sa
         assert k1.dtype == torch.uint8 and k1.shape == (T, B, 256) and k2.shape == (T, B, 128)
         assert k1.is_contiguous() and k2.is_contiguous()
         t["keep1"], t["keep2"] = k1, k2
-    if window is not None:
+    if window is not None or hold is not None:
         t["peak"] = rt.buf(sc.name("peak"), (B, T), torch.int32)
-    decoder_fwd_launches(lib, plan, w, t, mode, T, r, ks, max_ctas, L.current_stream(), window)
+    if hold is not None:
+        t["stop_at"] = stop_at
+        t["end_step"] = rt.buf(sc.name("end_step"), (B,), torch.int32)
+    decoder_fwd_launches(lib, plan, w, t, mode, T, r, ks, max_ctas, L.current_stream(), window, hold)
+    if hold is not None:
+        return y, align, t["peak"], t["end_step"]
     return (y, align) if window is None else (y, align, t["peak"])

@@ -65,6 +65,11 @@ class Config(object):
     # back >= 0, ahead >= 1: step t attends only positions p(t-1) - back .. p(t-1) + ahead around the previous step's
     # attention peak p(t-1) (p(-1) = 0).  Off by default, as in the reference; each call also sets attention_peaks.
     attention_window = None
+    # end-of-text stop rule at synthesis (free-running decoding; training never uses it): None = off, or hold >= 1: a row
+    # ends once `hold` consecutive steps have their attention peak at or past its last real character; each row group of
+    # 8 stops decoding soon after its last row ends, and inference returns only the steps the batch needed (end_steps).
+    # 4 steps is a starting point only: no value has been validated on a trained model.
+    stop_at_end = None
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -86,6 +91,7 @@ class Tacotron(object):
             from .. import kernels as K
             ops.decoder_budget(K.decoder_capacity()[0], max_ctas)
         ops.attention_window(getattr(config, "attention_window", None))     # a malformed window fails here too
+        ops.stop_rule_hold(getattr(config, "stop_at_end", None))            # and a malformed stop rule hold
         self.config = config
         self.train = train
         self.device = torch.device(device)
@@ -96,6 +102,7 @@ class Tacotron(object):
         self.global_step = 0
         self.seq2seq_output = self.output = self.alignments = self.loss = None
         self.attention_peaks = None               # int32 [B, T] peak position of each decoder step (attention window on)
+        self.end_steps = None                     # int32 [B] end_step of each row (stop rule on), on the device
         self.guided_attention_loss = None
         self.step_ns = None
         self.section_wait = None
@@ -126,7 +133,8 @@ class Tacotron(object):
                        sample_mask=None):
         """Returns a zero-argument callable that runs the whole decode (the BasicDecoder +
         dynamic_decode pair of the reference) as one persistent kernel: (seq2seq_output, alignments), and the step
-        peaks int32 [B, T] third when config.attention_window is set and train is False."""
+        peaks int32 [B, T] third when config.attention_window or config.stop_at_end is set and train is False, and
+        end_step int32 [B] fourth when config.stop_at_end is set (ops.attention_decoder)."""
         cfg = self.config
         if train:
             mel = inputs["mel"]
@@ -149,6 +157,7 @@ class Tacotron(object):
             dec_drop_masks = None
             sample_mask = None
         window = None if train else ops.attention_window(getattr(cfg, "attention_window", None))
+        hold = None if train else ops.stop_rule_hold(getattr(cfg, "stop_at_end", None))
         sc = ops.Scope(self.store, "dec")
         step_ns = self.step_ns
         if speaker_embed is not None and not getattr(cfg, "speaker_decoder", False):
@@ -158,10 +167,12 @@ class Tacotron(object):
             h0 = att0 = None
             if speaker_embed is not None:                     # initial attention vector and GRU states (tacotron.py:96-97)
                 _, h0, att0 = ops.decoder_speaker_state(sc, speaker_embed)
+            stop_at = None if hold is None else ops.stop_positions(inputs["text"], inputs["text_length"])
             return ops.attention_decoder(encoded, inputs["text_length"], cfg.r, T, mode=mode, mel=mel,
                                          sample_mask=sample_mask, drop_masks=dec_drop_masks,
                                          dropout=cfg.audio_dropout_prob, scope=sc, step_ns=step_ns,
-                                         max_ctas=getattr(cfg, "max_ctas", None), h0=h0, att0=att0, window=window)
+                                         max_ctas=getattr(cfg, "max_ctas", None), h0=h0, att0=att0, window=window,
+                                         stop_hold=hold, stop_at=stop_at)
         return run
 
     # -- inference (tacotron.py:107-154) --------------------------------------------------------
@@ -220,6 +231,9 @@ class Tacotron(object):
                   trace=None):
         """inputs: dict of CUDA tensors: 'text' int32 [B,Tx], 'text_length' int32 [B]; train adds
         'mel' fp32 [B,T,80r] (and 'stft' for the loss).  Returns (seq2seq_output, output).
+        With config.stop_at_end (not train) the decode stops at the end of the text: end_step is read once, the call
+        keeps T' = min(T, 4 ceil(max_b end_step / 4)) steps (ops.stopped_steps), runs the post-net on those only and
+        returns [B, T', ...] outputs; self.end_steps holds end_step.
         With config.cuda_graph the three sections (encoder / decoder / post-net) of an inference-mode call are
         captured once per input shape and replayed: ~26 launches collapse into 3 graph launches."""
         text = inputs["text"]
@@ -238,15 +252,21 @@ class Tacotron(object):
         res = dec()
         seq2seq_output, self.alignments = res[:2]
         self.attention_peaks = res[2] if len(res) > 2 else None
+        self.end_steps = res[3] if len(res) > 3 else None
         self._mark("decoder")
+        if self.end_steps is not None:                            # stop rule: the steps the batch needed
+            Tp = ops.stopped_steps(self.end_steps, seq2seq_output.shape[1])
+            seq2seq_output = seq2seq_output[:, :Tp].contiguous()
+            self.alignments, self.attention_peaks = self.alignments[:, :Tp], self.attention_peaks[:, :Tp]
         output = self._postnet(seq2seq_output, trace)
         self._mark("postnet")
         return seq2seq_output, output
 
     def _inference_graphed(self, inputs, T):
         T = self.config.max_decode_iter if T is None else T
+        hold = ops.stop_rule_hold(getattr(self.config, "stop_at_end", None))
         key = (tuple(inputs["text"].shape), T, self.store.version, getattr(self.config, "max_ctas", None),
-               ops.attention_window(getattr(self.config, "attention_window", None)))
+               ops.attention_window(getattr(self.config, "attention_window", None)), hold)
         g = self._graphs.get(key) if hasattr(self, "_graphs") else None
         if g is None:
             if not hasattr(self, "_graphs"):
@@ -274,10 +294,15 @@ class Tacotron(object):
                     res = dec()
                     outs["y"], outs["align"] = res[:2]
                     outs["peak"] = res[2] if len(res) > 2 else None
-                gp = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(gp, pool=pool):
-                    outs["out"] = self._postnet(outs["y"], None)
-                graphs = [ge, gd, gp]
+                    outs["end_step"] = res[3] if len(res) > 3 else None
+                graphs = [ge, gd]
+                if hold is None:
+                    gp = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(gp, pool=pool):
+                        outs["out"] = self._postnet(outs["y"], None)
+                    graphs.append(gp)
+                else:                                               # post-net graphs per kept length T', on demand
+                    outs["post"] = {}
             finally:
                 self._marks = marks
                 self.config.cuda_graph = cg_flag
@@ -301,11 +326,36 @@ class Tacotron(object):
         graphs[1].replay(); self._mark("decoder")
         if waits.get("postnet") is not None:
             cur.wait_event(waits["postnet"])
-        graphs[2].replay(); self._mark("postnet")
         self.alignments = outs["align"]
         self.attention_peaks = outs["peak"]
+        self.end_steps = outs["end_step"]
         self.last_graph_kernels = g[3]
-        return outs["y"], outs["out"]
+        if self.end_steps is None:
+            graphs[2].replay(); self._mark("postnet")
+            return outs["y"], outs["out"]
+        Tp = ops.stopped_steps(self.end_steps, T)
+        post = outs["post"].get(Tp)
+        if post is None:
+            post = outs["post"][Tp] = self._capture_postnet(outs["y"], Tp)
+        post[0].replay(); self._mark("postnet")
+        self.alignments, self.attention_peaks = self.alignments[:, :Tp], self.attention_peaks[:, :Tp]
+        return post[1], post[2]
+
+    def _capture_postnet(self, y, Tp):
+        """(graph, seq2seq_output [B, Tp, 80r], output) for the stop rule's graphed path: the first Tp steps of the
+        decoder graph's output y, copied to a static buffer, and the post-net on them (warmed up eagerly first, so
+        every scratch buffer of that length exists before the capture)"""
+        marks, self._marks = self._marks, None
+        try:
+            self._postnet(y[:, :Tp].contiguous(), None)
+            torch.cuda.synchronize()
+            gp = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(gp):
+                ys = y[:, :Tp].contiguous()
+                out = self._postnet(ys, None)
+        finally:
+            self._marks = marks
+        return gp, ys, out
 
     # -- add_loss_op (tacotron.py:156-165) -------------------------------------------------------
     def add_loss_op(self, seq2seq_output, output, mel, linear):

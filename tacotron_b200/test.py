@@ -44,6 +44,17 @@ fall far back or stick past the text.  It applies to every decode of the run, wi
 ``--trim-tail``, ``-s``, ``--max-ctas`` and ``--summaries``; the files written are the same ones.  The default 2,5 is
 close to the windows of common open Tacotron implementations and is a starting point only: no value has been tried on
 a trained model here.  Without the flag the decoder is the reference's.
+
+    python -m tacotron_b200.test -t nancy --stop-at-end               # hold 4
+    python -m tacotron_b200.test -t nancy --stop-at-end 3 --trim-tail
+
+``--stop-at-end [HOLD]`` stops decoding at the end of the text instead of after ``max_decode_iter`` steps: an utterance
+ends once HOLD consecutive decoder steps attend most to its last character or past it, each group of 8 utterances stops
+decoding a few steps after its last one ends, and the post-net and Griffin-Lim run only on the steps that were decoded.
+The WAV, the attention array and the summaries end at the stop (with ``--trim-tail`` also where the speech ends, if
+that comes first; with ``--long-form`` a chunk whose rule fired is never split again).  It works with every other flag.
+The default hold of 4 steps is a starting point only: no value has been tried on a trained model here.  An utterance
+whose attention never reaches the end of its text decodes all ``max_decode_iter`` steps, as without the flag.
 """
 from __future__ import annotations
 
@@ -58,8 +69,9 @@ import torch
 def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, trim_tail=False, long_form=False):
     """summary_dir: also write each prompt's audio and attention image as TensorBoard summaries there, at step 0
     (tacotron_b200/summary.py).  trim_tail: end each utterance where its speech ends; long_form: speak each line as one
-    clip, whatever its length (module docstring).  config.attention_window (None or (back, ahead)) applies to every
-    decode, plain and long-form.  Returns one device waveform per prompt."""
+    clip, whatever its length (module docstring).  config.attention_window (None or (back, ahead)) and
+    config.stop_at_end (None or a hold) apply to every decode, plain and long-form.  Returns one device waveform per
+    prompt."""
     from . import audio, checkpoint, data_input
     from .train import write_wav
     sr = 24000 if "blizzard" in config.data_path else 16000                              # test.py:15
@@ -117,8 +129,11 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, tri
             _, outputs = model.inference(inputs, train=False)
             alignments = model.alignments
             log("saving samples")
-            if trim_tail:
-                frames = audio.speech_frames(outputs, config.r, stft_mean=mean_d, stft_std=std_d)
+            steps = None
+            if trim_tail or model.end_steps is not None:
+                frames = audio.speech_frames(outputs, config.r, stft_mean=mean_d, stft_std=std_d) if trim_tail else None
+                if model.end_steps is not None:                                          # the stop rule's frames
+                    frames = audio.stop_frames(model.end_steps, config.r, outputs.shape[1], frames)
                 wav = audio.invert_speech(outputs, config.r, frames, stft_mean=mean_d, stft_std=std_d)
                 steps = (frames.cpu() // config.r).tolist()
             else:
@@ -126,7 +141,7 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, tri
             for b in range(outputs.shape[0]):                                            # :59-70
                 text = "".join(ivocab[int(w)] for w in inputs["text"][b].cpu().numpy())
                 wave, alignment = wav[b].cpu().numpy(), alignments[b].cpu().numpy()
-                if trim_tail:
+                if steps is not None:
                     alignment = alignment[:steps[b]]
                 write_wav(os.path.join(out_dir, f"{n}.wav"), wave, sr)
                 np.save(os.path.join(out_dir, f"{n}_attention.npy"), alignment)
@@ -162,14 +177,24 @@ def _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, 
             if config.num_speakers > 1:
                 inputs["speaker"] = torch.full((len(group),), speaker, dtype=torch.int32, device=inputs["text"].device)
             _, outputs = model.inference(inputs, train=False)
-            bounds = audio.speech_bounds(outputs, r, stft_mean=mean_d, stft_std=std_d).cpu().numpy()    # the one read
+            bounds = audio.speech_bounds(outputs, r, stft_mean=mean_d, stft_std=std_d)
+            fired = None
+            if model.end_steps is not None:  # stop rule: every chunk's bounds end at its stop (a no-op where it did not fire)
+                stop = audio.stop_frames(model.end_steps, r, outputs.shape[1])
+                f1 = torch.minimum(bounds[:, 1], stop)
+                bounds = torch.stack([torch.minimum(bounds[:, 0], f1), f1, torch.minimum(bounds[:, 2], stop),
+                                      (model.end_steps < config.max_decode_iter).to(torch.int32)], dim=1)
+            bounds = bounds.cpu().numpy()    # the one read
+            if bounds.shape[1] == 4:
+                bounds, fired = bounds[:, :3], bounds[:, 3] != 0
             y, start = audio.invert_speech_packed(outputs, r, bounds[:, 2], stft_mean=mean_d, stft_std=std_d)
             align = model.alignments.cpu().numpy()
             n = 4 * r * (outputs.shape[1] // 4)
             outs.append(y)
             for b, c in enumerate(group):
                 f0, f1, frames = (int(v) for v in bounds[b])
-                if f1 == n:                  # speech up to the last frame: most likely out of decoder steps
+                if f1 == n and (fired is None or not fired[b]):    # speech up to the last frame: most likely out of
+                                                                   # decoder steps
                     halves = longform.resplit(c)
                     if halves is not None:
                         cs = lines[c.line]
@@ -232,6 +257,17 @@ def parse_attention_window(text):
     return back, ahead
 
 
+def parse_stop_hold(text):
+    """'HOLD' -> an int >= 1 (the --stop-at-end value)"""
+    try:
+        hold = int(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"{text!r}: expected HOLD, an integer number of decoder steps such as 4") from None
+    if hold < 1:
+        raise argparse.ArgumentTypeError(f"{text!r}: HOLD must be >= 1")
+    return hold
+
+
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", "--train-set", default="nancy")
@@ -248,6 +284,9 @@ def main(argv=None):
                         metavar="BACK,AHEAD",
                         help="attend only BACK characters behind to AHEAD ahead of the previous step's attention peak "
                              "(a bare flag: 2,5, a starting point only)")
+    parser.add_argument("--stop-at-end", type=parse_stop_hold, nargs="?", const=4, default=None, metavar="HOLD",
+                        help="stop decoding once HOLD consecutive steps attend to the last character of the text or "
+                             "past it (a bare flag: 4, a starting point only)")
     args = parser.parse_args(argv)
     prompts = [p for p in sys.stdin.readlines() if len(p) > 0]                           # test.py:77-78
     from .models.tacotron import Config, Tacotron
@@ -256,6 +295,7 @@ def main(argv=None):
     config.save_path = args.train_set + "/tacotron"                                      # :84
     config.max_ctas = args.max_ctas
     config.attention_window = args.attention_window
+    config.stop_at_end = args.stop_at_end
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "test") if args.summaries else None      # test.py:33
     test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir, trim_tail=args.trim_tail,
