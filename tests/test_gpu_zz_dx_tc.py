@@ -1,10 +1,9 @@
 """GPU tests of the opt-in wgmma route for data gradients (kernels.DX_TC / Config.grad_dx_tc): a conv1d('same') data
 gradient is itself a convolution of dZ with the taps reversed and the weights transposed, so it can run on the forward's
-tensor-core kernel (taco_linear_fwd).  Single-pass TF32 like the forward: 3e-3 of max|ref| per call; whole-model
-gradients are held to the global bar of the TF32 forward test (relative L2 <= 0.15, cosine >= 0.98).
-
-STATUS (round 1): written after the round's GPU budget was spent -- no hardware run yet (non-strict xfail; the route is
-off by default)."""
+tensor-core kernel (taco_linear_fwd).  These per-call checks run the 3xTF32 route (DX_TC_IMPL's default) against the
+single-pass bar of 3e-3 of max|ref|; tests/test_gpu_zz_bwd_tc_envelope.py holds both DX_TC_IMPL values to per-element
+float64 bars.  The whole-model test runs Config.grad_dx_tc in 'tf32' mode (single-pass TF32 data gradients) and holds
+the gradients to the global bar of the TF32 forward test (relative L2 <= 0.15, cosine >= 0.98)."""
 import pytest
 import torch
 
