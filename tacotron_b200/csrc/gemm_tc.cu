@@ -63,8 +63,18 @@ struct SmemLayout {
     static_assert(TOTAL <= 227 * 1024, "shared memory per block exceeds 227 KB");
 };
 
-// fp32 -> nearest TF32-representable value (ties away from zero), two integer instructions
+// fp32 -> nearest TF32-representable value (ties away from zero), two integer instructions.  Adding 0x1000 carries the
+// canonical NaN 0x7fffffff (what GPU arithmetic produces) into the sign bit: that NaN becomes -0.  Used for the lo half
+// of a split, where the hi half carries any NaN.
 __device__ __forceinline__ float rn_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
+
+// rn_tf32 for the hi half of a split: the signed max (one VIADDMNMX in place of the add) returns a positive NaN as a NaN,
+// so a NaN computed by one layer stays NaN in the next contraction.  Every non-NaN value (infinities included) and every
+// negative NaN but 0xfffff000..0xffffffff, which arithmetic does not produce, rounds exactly as rn_tf32.
+__device__ __forceinline__ float rn_tf32_hi(float x) {
+    const uint32_t u = __float_as_uint(x);
+    return __uint_as_float((uint32_t)max((int)(u + 0x1000u), (int)u) & 0xffffe000u);
+}
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -184,7 +194,7 @@ __global__ void __launch_bounds__(TC_THREADS, MODE == 1 ? 1 : 2) gemm_tc_kernel(
                     const int r = frow + 8 * (e & 1);
                     const int c = 8 * k + tg + 4 * (e >> 1);
                     const float x = *reinterpret_cast<const float*>(As + r * 128 + (((c >> 2) ^ (r & 7)) << 4) + (c & 3) * 4);
-                    const float hv = rn_tf32(x);
+                    const float hv = rn_tf32_hi(x);
                     ah[k][e] = __float_as_uint(hv);
                     al[k][e] = __float_as_uint(rn_tf32(x - hv));
                 }
@@ -637,10 +647,10 @@ __global__ void __launch_bounds__(DW_THREADS, 1) dw_tc_kernel(const __grid_const
             for (int kc = kc0; kc < kc0 + 4; ++kc) {
                 float4 h4, l4;
                 const float z0 = zs[(4 * kc + 0) * 128 + cn], z1 = zs[(4 * kc + 1) * 128 + cn], z2 = zs[(4 * kc + 2) * 128 + cn], z3 = zs[(4 * kc + 3) * 128 + cn];
-                h4.x = rn_tf32(z0); l4.x = rn_tf32(z0 - h4.x);
-                h4.y = rn_tf32(z1); l4.y = rn_tf32(z1 - h4.y);
-                h4.z = rn_tf32(z2); l4.z = rn_tf32(z2 - h4.z);
-                h4.w = rn_tf32(z3); l4.w = rn_tf32(z3 - h4.w);
+                h4.x = rn_tf32_hi(z0); l4.x = rn_tf32(z0 - h4.x);
+                h4.y = rn_tf32_hi(z1); l4.y = rn_tf32(z1 - h4.y);
+                h4.z = rn_tf32_hi(z2); l4.z = rn_tf32(z2 - h4.z);
+                h4.w = rn_tf32_hi(z3); l4.w = rn_tf32(z3 - h4.w);
                 const int off = cn * 128 + ((kc ^ (cn & 7)) << 4);
                 *reinterpret_cast<float4*>(zconv + off) = h4;
                 *reinterpret_cast<float4*>(zconv + DW_TILE_BYTES + off) = l4;
@@ -654,7 +664,7 @@ __global__ void __launch_bounds__(DW_THREADS, 1) dw_tc_kernel(const __grid_const
     #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const float x = xs[(8 * k + tg + 4 * (e >> 1)) * 128 + mrow + 8 * (e & 1)];
-                    const float hv = rn_tf32(x);
+                    const float hv = rn_tf32_hi(x);
                     ah[k][e] = __float_as_uint(hv);
                     al[k][e] = __float_as_uint(rn_tf32(x - hv));
                 }
@@ -814,7 +824,7 @@ __global__ void __launch_bounds__(HS_THREADS, 1) highway_stack_kernel(const __gr
                     const int r = frow + 8 * (e & 1);
                     const int c = 8 * k + tg + 4 * (e >> 1);
                     const float x = *reinterpret_cast<const float*>(As + r * 128 + (((c >> 2) ^ (r & 7)) << 4) + (c & 3) * 4);
-                    const float hv = rn_tf32(x);
+                    const float hv = rn_tf32_hi(x);
                     ah[k][e] = __float_as_uint(hv);
                     al[k][e] = __float_as_uint(rn_tf32(x - hv));
                 }
