@@ -113,35 +113,95 @@ class TacoError(RuntimeError):
 
 _lib = None
 
-# every symbol include/taco_b200.h declares (tests check the .so exports all of them)
-EXPORTS = [
-    "taco_last_error", "taco_version", "taco_device_info", "taco_linear_fwd", "taco_linear_route", "taco_pack_weight",
-    "taco_pack_weight_x3", "taco_highway_stack_fwd",
-    "taco_maxpool_fwd", "taco_gather_rows", "taco_mask_rows", "taco_bigru_fwd", "taco_bigru_fwd_h0",
-    "taco_decoder_packed_bytes", "taco_decoder_workspace_bytes", "taco_decoder_trace_offset", "taco_decoder_pack",
-    "taco_decoder_fwd",
-    "taco_decoder_capacity",
-    "taco_l1_loss_fwd", "taco_l1_partial_count", "taco_launch_count",
+vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
+
+# every symbol include/taco_b200.h declares -> (restype, argtypes); tests check that the .so exports exactly these
+SIGNATURES = {
+    "taco_last_error": (C.c_char_p, []),
+    "taco_version": (i32, []),
+    "taco_device_info": (i32, [C.POINTER(C.c_int)] * 3),
+    "taco_linear_fwd": (i32, [C.POINTER(LinearDesc), vp]),
+    "taco_linear_route": (i32, [C.POINTER(LinearDesc)] + [C.POINTER(C.c_int)] * 5),
+    "taco_pack_weight": (i32, [vp, i32, i32, i32, vp, i64, vp]),
+    "taco_pack_weight_x3": (i32, [vp, i32, i32, i32, vp, vp, i64, vp]),
+    "taco_highway_stack_fwd": (i32, [C.POINTER(HighwayStackDesc), vp]),
+    "taco_maxpool_fwd": (i32, [vp, vp, i32, i32, i32, vp]),
+    "taco_gather_rows": (i32, [vp, vp, i32, i32, i32, vp, f32, vp, vp]),
+    "taco_mask_rows": (i32, [vp, vp, vp, i32, i32, i32, vp]),
+    "taco_bigru_fwd": (i32, [vp] * 6 + [i32, i32, vp]),
+    "taco_bigru_fwd_h0": (i32, [vp] * 8 + [i32, i32, vp]),
+    "taco_decoder_packed_bytes": (C.c_size_t, [i32]),
+    "taco_decoder_workspace_bytes": (C.c_size_t, [i32] * 4),
+    "taco_decoder_trace_offset": (i64, []),
+    "taco_decoder_pack": (i32, [C.POINTER(DecoderWeights), i32, vp, vp]),
+    "taco_decoder_fwd": (i32, [C.POINTER(DecoderArgs), vp]),
+    "taco_decoder_capacity": (i32, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "taco_l1_loss_fwd": (i32, [vp, vp, i64, vp, vp, vp]),
+    "taco_l1_partial_count": (i32, []),
+    "taco_launch_count": (C.c_ulonglong, []),
     # training path
-    "taco_gemm", "taco_set_gemm_impl", "taco_conv_dw", "taco_colsum", "taco_colsum_seg", "taco_bias_act", "taco_mul_shift", "taco_epi_bwd", "taco_epi_fwd_keep", "taco_bn_param_grad",
-    "taco_maxpool_bwd", "taco_highway_fwd", "taco_highway_bwd", "taco_l1_bwd", "taco_l1_bwd_ld", "taco_scatter_add_rows", "taco_bigru_bwd", "taco_bigru_bwd_h0",
-    "taco_dec_inputs", "taco_decoder_bwd_workspace_bytes", "taco_decoder_bwd", "taco_attn_bwd_post", "taco_sumsq",
-    "taco_adam_step",
+    "taco_gemm": (i32, [C.POINTER(GemmDesc), vp]),
+    "taco_set_gemm_impl": (i32, [i32]),
+    "taco_conv_dw": (i32, [vp, i64, i64, vp, i64, vp, i64] + [C.c_int32] * 6 + [vp]),
+    "taco_colsum": (i32, [vp, vp, i64, vp, i64, vp, i64, i32, i32, vp]),
+    "taco_colsum_seg": (i32, [vp, i64, vp, i64, i32, i32, i32, vp]),
+    "taco_bias_act": (i32, [vp, i64, i32, i32, vp, i32, vp]),
+    "taco_mul_shift": (i32, [vp, i64, vp, i64, vp, i64, i32, i32, i32, i32, vp]),
+    "taco_epi_bwd": (i32, [vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, i32, vp, vp, f32, vp]),
+    "taco_epi_fwd_keep": (i32, [vp, i64, vp, i32, i32, f32, vp]),
+    "taco_bn_param_grad": (i32, [vp, vp, vp, vp, vp, vp, i32, vp]),
+    "taco_maxpool_bwd": (i32, [vp, vp, vp, i32, i32, i32, vp]),
+    "taco_highway_fwd": (i32, [vp, i64, vp, i64, vp, i64, i32, i32, vp]),
+    "taco_highway_bwd": (i32, [vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, vp]),
+    "taco_l1_bwd": (i32, [vp, vp, vp, i64, f32, vp]),
+    "taco_l1_bwd_ld": (i32, [vp, i64, vp, vp, i64, i64, f32, vp]),
+    "taco_scatter_add_rows": (i32, [vp, vp, vp, i32, i32, i32, vp]),
+    "taco_bigru_bwd": (i32, [vp] * 8 + [i32, i32, vp]),
+    "taco_bigru_bwd_h0": (i32, [vp] * 11 + [i32, i32, vp]),
+    "taco_dec_inputs": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+    "taco_decoder_bwd_workspace_bytes": (C.c_size_t, []),
+    "taco_decoder_bwd": (i32, [C.POINTER(DecoderBwdArgs), vp]),
+    "taco_attn_bwd_post": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]),
+    "taco_sumsq": (i32, [vp, i64, vp, vp, vp]),
+    "taco_adam_step": (i32, [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp, vp]),
     # guided attention loss (opt-in training term)
-    "taco_guided_attention", "taco_guided_attention_partial_count",
+    "taco_guided_attention": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, vp, vp]),
+    "taco_guided_attention_partial_count": (i32, [i32, i32]),
     # spectrogram inversion (Griffin-Lim glue kernels)
-    "taco_gl_init", "taco_gl_ola", "taco_gl_frame", "taco_gl_phase", "taco_rfft2048", "taco_irfft2048",
+    "taco_gl_init": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]),
+    "taco_gl_ola": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
+    "taco_gl_frame": (i32, [vp, vp, i32, i32, i32, i32, i32, vp]),
+    "taco_gl_phase": (i32, [vp, vp, vp, i64, vp]),
+    "taco_rfft2048": (i32, [vp, vp, i64, vp]),
+    "taco_irfft2048": (i32, [vp, vp, i64, vp]),
     # end of speech and the packed Griffin-Lim kernels (synthesis tail trim)
-    "taco_speech_frames", "taco_gl_init_packed", "taco_gl_ola_packed", "taco_gl_frame_packed",
+    "taco_speech_frames": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]),
+    "taco_gl_init_packed": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]),
+    "taco_gl_ola_packed": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+    "taco_gl_frame_packed": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     # where speech starts and ends, and the join of synthesised pieces (long-form synthesis)
-    "taco_speech_bounds", "taco_join_segments",
+    "taco_speech_bounds": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]),
+    "taco_join_segments": (i32, [vp, i64, vp, vp, i32, i32, i32, vp]),
     # input data format
-    "taco_normalize_f16",
+    "taco_normalize_f16": (i32, [vp, vp, vp, vp, i64, i32, vp]),
     # feature extraction (preprocessing)
-    "taco_trim_bounds", "taco_feature_frames", "taco_feature_spec", "taco_resample",
+    "taco_trim_bounds": (i32, [vp, vp, vp, i32, i32, i32, f32, vp]),
+    "taco_feature_frames": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]),
+    "taco_feature_spec": (i32, [vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+    "taco_resample": (i32, [vp, vp, vp, vp, i32, vp, i32, i32, C.c_double, vp, i64, vp]),
     # training summaries
-    "taco_histogram_workspace_bytes", "taco_histogram",
-]
+    "taco_histogram_workspace_bytes": (C.c_size_t, []),
+    "taco_histogram": (i32, [vp, i64, vp, i32, vp, vp, vp, vp, vp]),
+}
+EXPORTS = list(SIGNATURES)
+
+
+def declare(cdll, names=EXPORTS):
+    """Give each named entry point of cdll (this library, or a build of the same sources) its SIGNATURES entry."""
+    for name in names:
+        fn = getattr(cdll, name)                  # a symbol that does not resolve raises AttributeError
+        fn.restype, fn.argtypes = SIGNATURES[name]
+    return cdll
 
 
 def lib():
@@ -153,83 +213,8 @@ def lib():
         raise TacoError(
             f"{LIB_PATH} not found: the CUDA extension has not been built (run `python -m tacotron_b200.build` "
             "or __graft_entry__.build()). There is no CPU fallback.")
-    L = C.CDLL(LIB_PATH)
-    L.taco_last_error.restype = C.c_char_p
-    L.taco_version.restype = C.c_int
-    L.taco_device_info.argtypes = [C.POINTER(C.c_int)] * 3
-    L.taco_linear_fwd.argtypes = [C.POINTER(LinearDesc), C.c_void_p]
-    L.taco_linear_route.argtypes = [C.POINTER(LinearDesc)] + [C.POINTER(C.c_int)] * 5
-    L.taco_pack_weight.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
-    L.taco_conv_dw.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64] + [C.c_int32] * 6 + [C.c_void_p]
-    L.taco_pack_weight_x3.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
-    L.taco_highway_stack_fwd.argtypes = [C.POINTER(HighwayStackDesc), C.c_void_p]
-    L.taco_maxpool_fwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    L.taco_gather_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_float,
-                                   C.c_void_p, C.c_void_p]
-    L.taco_mask_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    L.taco_bigru_fwd.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p]
-    L.taco_bigru_fwd_h0.argtypes = [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_void_p]
-    L.taco_decoder_packed_bytes.argtypes = [C.c_int]
-    L.taco_decoder_packed_bytes.restype = C.c_size_t
-    L.taco_decoder_workspace_bytes.argtypes = [C.c_int] * 4
-    L.taco_decoder_workspace_bytes.restype = C.c_size_t
-    L.taco_decoder_trace_offset.argtypes = []
-    L.taco_decoder_trace_offset.restype = C.c_int64
-    L.taco_decoder_pack.argtypes = [C.POINTER(DecoderWeights), C.c_int, C.c_void_p, C.c_void_p]
-    L.taco_decoder_fwd.argtypes = [C.POINTER(DecoderArgs), C.c_void_p]
-    L.taco_decoder_capacity.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    L.taco_l1_loss_fwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.taco_l1_partial_count.restype = C.c_int
-    L.taco_launch_count.restype = C.c_ulonglong
-    vp, i64, i32, f32 = C.c_void_p, C.c_int64, C.c_int, C.c_float
-    L.taco_gemm.argtypes = [C.POINTER(GemmDesc), vp]
-    L.taco_colsum.argtypes = [vp, vp, i64, vp, i64, vp, i64, i32, i32, vp]
-    L.taco_colsum_seg.argtypes = [vp, i64, vp, i64, i32, i32, i32, vp]
-    L.taco_bias_act.argtypes = [vp, i64, i32, i32, vp, i32, vp]
-    L.taco_mul_shift.argtypes = [vp, i64, vp, i64, vp, i64, i32, i32, i32, i32, vp]
-    L.taco_epi_bwd.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, i32, vp, vp, f32, vp]
-    L.taco_epi_fwd_keep.argtypes = [vp, i64, vp, i32, i32, f32, vp]
-    L.taco_bn_param_grad.argtypes = [vp, vp, vp, vp, vp, vp, i32, vp]
-    L.taco_maxpool_bwd.argtypes = [vp, vp, vp, i32, i32, i32, vp]
-    L.taco_highway_fwd.argtypes = [vp, i64, vp, i64, vp, i64, i32, i32, vp]
-    L.taco_highway_bwd.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, vp]
-    L.taco_l1_bwd.argtypes = [vp, vp, vp, i64, f32, vp]
-    L.taco_l1_bwd_ld.argtypes = [vp, i64, vp, vp, i64, i64, f32, vp]
-    L.taco_scatter_add_rows.argtypes = [vp, vp, vp, i32, i32, i32, vp]
-    L.taco_bigru_bwd.argtypes = [vp] * 8 + [i32, i32, vp]
-    L.taco_bigru_bwd_h0.argtypes = [vp] * 11 + [i32, i32, vp]
-    L.taco_dec_inputs.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
-    L.taco_decoder_bwd_workspace_bytes.restype = C.c_size_t
-    L.taco_decoder_bwd.argtypes = [C.POINTER(DecoderBwdArgs), vp]
-    L.taco_attn_bwd_post.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]
-    L.taco_sumsq.argtypes = [vp, i64, vp, vp, vp]
-    L.taco_adam_step.argtypes = [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp, vp]
-    L.taco_guided_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, vp, vp]
-    L.taco_guided_attention_partial_count.argtypes = [i32, i32]
-    L.taco_guided_attention_partial_count.restype = C.c_int
-    L.taco_gl_init.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
-    L.taco_gl_ola.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]
-    L.taco_gl_frame.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]
-    L.taco_gl_phase.argtypes = [vp, vp, vp, i64, vp]
-    L.taco_rfft2048.argtypes = [vp, vp, i64, vp]
-    L.taco_irfft2048.argtypes = [vp, vp, i64, vp]
-    L.taco_speech_frames.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]
-    L.taco_gl_init_packed.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
-    L.taco_gl_ola_packed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
-    L.taco_gl_frame_packed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
-    L.taco_speech_bounds.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]
-    L.taco_join_segments.argtypes = [vp, i64, vp, vp, i32, i32, i32, vp]
-    L.taco_normalize_f16.argtypes = [vp, vp, vp, vp, i64, i32, vp]
-    L.taco_trim_bounds.argtypes = [vp, vp, vp, i32, i32, i32, f32, vp]
-    L.taco_feature_frames.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
-    L.taco_feature_spec.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
-    L.taco_resample.argtypes = [vp, vp, vp, vp, i32, vp, i32, i32, C.c_double, vp, i64, vp]
-    L.taco_histogram_workspace_bytes.restype = C.c_size_t
-    L.taco_histogram.argtypes = [vp, i64, vp, i32, vp, vp, vp, vp, vp]
-    for name in EXPORTS:                      # every declared symbol must resolve (AttributeError otherwise)
-        getattr(L, name)
-    _lib = L
-    return L
+    _lib = declare(C.CDLL(LIB_PATH))              # every declared symbol must resolve
+    return _lib
 
 
 def check(rc, what=""):

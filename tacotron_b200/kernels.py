@@ -17,8 +17,13 @@ from . import _lib as L
 ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH = 0, 1, 2, 3
 
 
+def _on_device(t):
+    """whether tensor t lives where the library's kernels run: every 'is a CUDA tensor' check goes through here"""
+    return t.is_cuda
+
+
 def _chk2(t, name):
-    if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and (t.shape[1] == 1 or t.stride(1) == 1)):
+    if not (_on_device(t) and t.dtype == torch.float32 and t.dim() == 2 and (t.shape[1] == 1 or t.stride(1) == 1)):
         raise L.TacoError(f"{name}: expected a CUDA fp32 [M,N] view with unit inner stride, got {tuple(t.shape)} "
                           f"{t.dtype} {t.device} strides {t.stride()}")
     return t
@@ -274,7 +279,7 @@ def scatter_add_rows(dTable, ids, dRows):
 def bigru_bwd(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw):
     B, T, _ = out.shape
     for t in (dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw):
-        assert t.is_contiguous() and t.is_cuda
+        assert t.is_contiguous() and _on_device(t)
     L.check(L.lib().taco_bigru_bwd(_p(dxp), _p(dOut), _p(out), _p(ACT), _p(Wg_h_fw), _p(Wc_h_fw), _p(Wg_h_bw), _p(Wc_h_bw), B, T,
                                    _st()), "taco_bigru_bwd")
 
@@ -282,7 +287,7 @@ def bigru_bwd(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw):
 def bigru_bwd_h0(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw, dh0):
     B, T, _ = out.shape
     for t in (dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw, dh0):
-        assert t is None or (t.is_contiguous() and t.is_cuda)
+        assert t is None or (t.is_contiguous() and _on_device(t))
     for t in (h0_fw, h0_bw):
         assert t is None or tuple(t.shape) == (B, 128)
     assert dh0 is None or tuple(dh0.shape) == (B, 2, 128)
@@ -293,7 +298,7 @@ def bigru_bwd_h0(dxp, dOut, out, ACT, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw,
 def bigru_fwd_h0(out, xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw):
     B, T, _ = out.shape
     for t in (out, xp, Wg_h_fw, Wc_h_fw, Wg_h_bw, Wc_h_bw, h0_fw, h0_bw):
-        assert t is None or (t.is_contiguous() and t.is_cuda)
+        assert t is None or (t.is_contiguous() and _on_device(t))
     for t in (h0_fw, h0_bw):
         assert t is None or tuple(t.shape) == (B, 128)
     L.check(L.lib().taco_bigru_fwd_h0(_p(xp), _p(Wg_h_fw), _p(Wc_h_fw), _p(Wg_h_bw), _p(Wc_h_bw), _p(h0_fw), _p(h0_bw), _p(out),
@@ -321,7 +326,7 @@ def decoder_bwd(a):
     d.B, d.T, d.Tx, d.r, d.keep_scale = B, T, Tx, OUT // 80, float(a["keep_scale"])
     for k in ("W_a", "W_q", "W_out", "W_in", "W1", "W2", "v", "dy_ext", "align", "values", "keys", "PQ", "PN1", "PN2", "sel",
               "DATT", "DY", "DPQ", "DSCORE", "DCTX", "DZ", "DPN2", "DPN1", "DX"):
-        assert a[k].is_contiguous() and a[k].is_cuda, k
+        assert a[k].is_contiguous() and _on_device(a[k]), k
         setattr(d, k, a[k].data_ptr())
     for k in ("Wg", "Wc", "RU", "C", "H", "DG", "DC"):
         for i in range(3):
@@ -329,13 +334,13 @@ def decoder_bwd(a):
             getattr(d, k)[i] = a[k][i].data_ptr()
     if a.get("H0") is not None:                              # initial GRU states h_i(-1) [B][256] (speaker-conditioned decoder)
         for i in range(3):
-            assert a["H0"][i].is_contiguous() and a["H0"][i].is_cuda and tuple(a["H0"][i].shape) == (B, 256)
+            assert a["H0"][i].is_contiguous() and _on_device(a["H0"][i]) and tuple(a["H0"][i].shape) == (B, 256)
             d.H0[i] = a["H0"][i].data_ptr()
     if a.get("DH0") is not None:                             # out: d(loss)/d(h_i(-1)) [3][B][256]
-        assert a["DH0"].is_contiguous() and a["DH0"].is_cuda and tuple(a["DH0"].shape) == (3, B, 256)
+        assert a["DH0"].is_contiguous() and _on_device(a["DH0"]) and tuple(a["DH0"].shape) == (3, B, 256)
         d.DH0 = a["DH0"].data_ptr()
     if a.get("dscore_add") is not None:                      # [B][T][Tx] added to every step's dscore (guided attention)
-        assert a["dscore_add"].is_contiguous() and a["dscore_add"].is_cuda and a["dscore_add"].shape == a["align"].shape
+        assert a["dscore_add"].is_contiguous() and _on_device(a["dscore_add"]) and a["dscore_add"].shape == a["align"].shape
         d.dscore_add = a["dscore_add"].data_ptr()
     ws = torch.empty(L.lib().taco_decoder_bwd_workspace_bytes() // 4, dtype=torch.float32, device=a["dy_ext"].device)
     d.workspace = ws.data_ptr()
@@ -388,7 +393,7 @@ def mask_rows(dst, src, length):
 
 # ---- Griffin-Lim glue (tacotron_b200/audio.py) ----
 def _f32c(t, name):
-    if not (t.is_cuda and t.is_contiguous() and t.dtype in (torch.float32, torch.complex64)):
+    if not (_on_device(t) and t.is_contiguous() and t.dtype in (torch.float32, torch.complex64)):
         raise L.TacoError(f"{name}: expected a contiguous CUDA fp32/complex64 tensor, got {t.dtype} {t.device}")
     return t
 
@@ -551,14 +556,14 @@ def gl_frame_packed(frw, y, off, max_frames, hop, win_length):
 def normalize_f16(out, x, mean, std):
     """out fp32 [..., W] = the reference's in-place float16 normalisation of x (float16) followed by the float32 cast"""
     W = x.shape[-1]
-    assert x.is_cuda and x.dtype == torch.float16 and x.is_contiguous() and out.dtype == torch.float32 and out.is_contiguous()
+    assert _on_device(x) and x.dtype == torch.float16 and x.is_contiguous() and out.dtype == torch.float32 and out.is_contiguous()
     assert mean.dtype == torch.float16 and std.dtype == torch.float32 and mean.numel() == W == std.numel() and out.shape == x.shape
     L.check(L.lib().taco_normalize_f16(_p(out), _p(x), _p(mean), _p(std), x.numel() // W, W, _st()), "taco_normalize_f16")
 
 
 # ---- feature extraction (tacotron_b200/audio.py process_audio_batch) ----
 def _cuda_c(t, dtype, name):
-    if not (t.is_cuda and t.is_contiguous() and t.dtype == dtype):
+    if not (_on_device(t) and t.is_contiguous() and t.dtype == dtype):
         raise L.TacoError(f"{name}: expected a contiguous CUDA {dtype} tensor, got {t.dtype} {t.device}")
     return t
 
@@ -642,6 +647,6 @@ def sumsq(out, x):
 
 def adam_step(p, g, m, v, lr_t, b1, b2, eps, clip, sumsq_t):
     for t in (p, g, m, v):
-        assert t.is_contiguous() and t.is_cuda and t.dtype == torch.float32
+        assert t.is_contiguous() and _on_device(t) and t.dtype == torch.float32
     L.check(L.lib().taco_adam_step(_p(p), _p(g), _p(m), _p(v), p.numel(), float(lr_t), float(b1), float(b2), float(eps),
                                    float(clip), _p(sumsq_t), _st()), "taco_adam_step")

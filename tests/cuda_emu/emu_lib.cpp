@@ -1,8 +1,7 @@
-// emu_lib.cpp -- TEST INFRASTRUCTURE ONLY.  Builds libtaco_emu.so: the product's own kernel sources (audio.cu, data.cu,
-// every kernel of train.cu) compiled with g++ over tests/cuda_emu/emu.h, exporting the SAME C-ABI entry points
-// (taco_gemm, taco_set_gemm_impl, taco_bias_act, ..., taco_gl_*, taco_normalize_f16) so that tests/test_cuda_emu.py and
-// tests/test_train_envelope_host.py can drive them through
-// ctypes with host pointers and compare with the torch-CPU mirrors -- no GPU involved.
+// emu_lib.cpp -- TEST INFRASTRUCTURE ONLY.  The library half of libtaco_emu.so: the error string and the launch counter
+// the product's kernel sources (the other emu_*.cpp units, one per .cu file) expect.  tests/emulator.py compiles all the
+// units for the host over tests/cuda_emu/emu.h and links them into one library exporting the SAME C-ABI entry points;
+// every test that takes its `emu` fixture drives them through ctypes with host pointers -- no GPU involved.
 #include "emu.h"
 
 #include <cstdarg>
@@ -18,5 +17,4 @@ void taco_set_error(const char* fmt, ...) {
 }
 extern "C" const char* taco_last_error(void) { return g_err; }
 
-// the kernel sources are compiled as separate translation units (their anonymous-namespace helpers share names):
-// emu_train.cpp, emu_audio.cpp, emu_data.cpp
+// the kernel sources are compiled as separate translation units (their anonymous-namespace helpers share names)

@@ -3,8 +3,8 @@ Griffin-Lim kernels (gl_init, gl_ola, gl_frame, gl_phase, padded and packed) of 
 (feature_frames, feature_spec) of csrc/features.cu.  Written once, run on the H100 by tests/test_gpu_z_stft_envelope.py
 and under the host emulation (tests/cuda_emu) by tests/test_stft_envelope_host.py.
 
-Every check takes an `Env`: a kernel namespace `K` (tacotron_b200.kernels, or `LibK` over the emulated library), the
-device and the stream.  Every reference is float64, computed from the kernel's own float32 operands -- in a chain, the
+Every check takes an `Env`: a kernel namespace `K` (tacotron_b200.kernels, over the device library or the emulated
+one), the device and the stream.  Every reference is float64, computed from the kernel's own float32 operands -- in a chain, the
 output of the previous kernel -- so every bar is local.  Outputs are prefilled with a sentinel bit pattern (NaN-like,
 never produced by arithmetic) and sit inside PAD elements of it that must survive; operands sit inside NaN bands.
 
@@ -75,65 +75,8 @@ def gen(seed):
     return torch.Generator().manual_seed(seed)
 
 
-# ------------------------------------------------------------------------------------------------------------------
-# the kernels over any C ABI (the emulated library on the host), with the signatures of tacotron_b200.kernels
-# ------------------------------------------------------------------------------------------------------------------
 def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
-
-
-class LibK:
-    def __init__(self, lib, stream=None):
-        self.lib, self.st = lib, stream
-
-    def _ok(self, rc, what):
-        assert rc == 0, f"{what}: {self.lib.taco_last_error().decode()}"
-
-    def gl_init(self, full, mag, spec, phase_u, r, scale=None, shift=None):
-        B, n, F = mag.shape
-        self._ok(self.lib.taco_gl_init(_p(full), _p(mag), _p(spec), _p(phase_u), B, spec.shape[1], n, r, F, _p(scale),
-                                       _p(shift), self.st), "taco_gl_init")
-
-    def gl_ola(self, y, fr, hop, win_length):
-        B, n, n_fft = fr.shape
-        self._ok(self.lib.taco_gl_ola(_p(y), _p(fr), B, n, hop, n_fft, win_length, self.st), "taco_gl_ola")
-
-    def gl_frame(self, frw, y, hop, win_length):
-        B, n, n_fft = frw.shape
-        self._ok(self.lib.taco_gl_frame(_p(frw), _p(y), B, n, hop, n_fft, win_length, self.st), "taco_gl_frame")
-
-    def gl_phase(self, full, mag, rebuilt):
-        self._ok(self.lib.taco_gl_phase(_p(full), _p(mag), _p(rebuilt), mag.numel(), self.st), "taco_gl_phase")
-
-    def rfft2048(self, X, x):
-        self._ok(self.lib.taco_rfft2048(_p(X), _p(x), x.numel() // N, self.st), "taco_rfft2048")
-
-    def irfft2048(self, x, X):
-        self._ok(self.lib.taco_irfft2048(_p(x), _p(X), x.numel() // N, self.st), "taco_irfft2048")
-
-    def gl_init_packed(self, full, mag, spec, phase_u, off, r, max_frames, scale=None, shift=None):
-        self._ok(self.lib.taco_gl_init_packed(_p(full), _p(mag), _p(spec), _p(phase_u), _p(off), off.numel() - 1,
-                                              spec.shape[1], r, mag.shape[1], int(max_frames), _p(scale), _p(shift),
-                                              self.st), "taco_gl_init_packed")
-
-    def gl_ola_packed(self, y, fr, off, max_frames, hop, win_length):
-        self._ok(self.lib.taco_gl_ola_packed(_p(y), _p(fr), _p(off), off.numel() - 1, int(max_frames), hop, fr.shape[1],
-                                             win_length, self.st), "taco_gl_ola_packed")
-
-    def gl_frame_packed(self, frw, y, off, max_frames, hop, win_length):
-        self._ok(self.lib.taco_gl_frame_packed(_p(frw), _p(y), _p(off), off.numel() - 1, int(max_frames), hop,
-                                               frw.shape[1], win_length, self.st), "taco_gl_frame_packed")
-
-    def feature_frames(self, frw, y, start, length, max_len, hop, win_length, preemph):
-        B, n, n_fft = frw.shape
-        self._ok(self.lib.taco_feature_frames(_p(frw), _p(y), _p(start), _p(length), B, n, max_len, hop, n_fft,
-                                              win_length, float(preemph), self.st), "taco_feature_frames")
-
-    def feature_spec(self, stft_out, mel_out, X, basis, lo, hi, r):
-        B, n, _ = X.shape
-        self._ok(self.lib.taco_feature_spec(_p(stft_out), _p(mel_out), int(stft_out.dtype == torch.float16), _p(X),
-                                            _p(basis), _p(lo), _p(hi), B, n, r, basis.shape[0], self.st),
-                 "taco_feature_spec")
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -5,59 +5,18 @@ T in {0..5, 7, 9} covers every tail of the forward's two-step loop and its prefe
 non-zero offsets.  The emulation computes the activations with expf and a true division, so the local bars use its
 own bounds: sigmoid within 2^-23 and tanh within 2^-22 (one rounding of the quotient and of 1 - quotient, plus expf's).
 """
-import ctypes as C
-import os
-import subprocess
-
 import pytest
 import torch
 
 from tests import bigru_envelope_checks as BG
+from tests.emulator import KernelsOver, emu  # noqa: F401  (the emulated library, built once per process)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-vp, i32 = C.c_void_p, C.c_int
 SHAPES = [(1, 0), (3, 0), (0, 5), (1, 1), (2, 1), (3, 2), (1, 3), (2, 4), (3, 5), (2, 7), (1, 9)]
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu_bigru_env") / "libtaco_emu_bigru_env.so")
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_gru.cpp", "emu_gru_bwd.cpp")]
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I",
-                           os.path.join(ROOT, "include"), *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_bigru_fwd_h0.argtypes = [vp] * 8 + [i32, i32, vp]           # as tacotron_b200/_lib.py declares them
-    lib.taco_bigru_bwd_h0.argtypes = [vp] * 11 + [i32, i32, vp]
-    return lib
-
-
-class EmuK:
-    """tacotron_b200.kernels.bigru_fwd_h0 / bigru_bwd_h0 over the emulated library, with host pointers"""
-
-    def __init__(self, lib):
-        self.lib = lib
-
-    def _check(self, rc, what):
-        assert rc == 0, f"{what}: {self.lib.taco_last_error().decode()}"
-
-    def bigru_fwd_h0(self, out, xp, Wg_fw, Wc_fw, Wg_bw, Wc_bw, h0_fw, h0_bw):
-        B, T, _ = out.shape
-        self._check(BG.fwd_call(BG.Env(self, self.lib, "cpu"), xp, [Wg_fw, Wc_fw, Wg_bw, Wc_bw], h0_fw, h0_bw, out, B, T),
-                    "taco_bigru_fwd_h0")
-
-    def bigru_bwd_h0(self, dxp, dOut, out, ACT, Wg_fw, Wc_fw, Wg_bw, Wc_bw, h0_fw, h0_bw, dh0):
-        B, T, _ = out.shape
-        self._check(BG.bwd_call(BG.Env(self, self.lib, "cpu"), dxp, dOut, out, ACT, [Wg_fw, Wc_fw, Wg_bw, Wc_bw], h0_fw,
-                                h0_bw, dh0, B, T), "taco_bigru_bwd_h0")
-
-
-@pytest.fixture(scope="module")
-def env(lib):
-    return BG.Env(EmuK(lib), lib, "cpu", None, eps_sig=2.0 ** -23, eps_tanh=2.0 ** -22)
+def env(emu):  # noqa: F811
+    return BG.Env(KernelsOver(emu), emu, "cpu", None, eps_sig=2.0 ** -23, eps_tanh=2.0 ** -22)
 
 
 def _cases():

@@ -1,5 +1,5 @@
-"""Functional check of CUDA kernels WITHOUT a GPU: the product's own kernel sources are compiled with g++ over
-tests/cuda_emu/emu.h (a thread-per-thread host emulation: real barriers, shuffles, a warp-collective mma defined from the
+"""Functional check of CUDA kernels WITHOUT a GPU: the product's own kernel sources are compiled for the host over
+tests/cuda_emu/emu.h by tests/emulator.py (a thread-per-thread host emulation: real barriers, shuffles, a warp-collective mma defined from the
 PTX fragment layout) and driven through the same C-ABI entry points with host pointers, against the torch-CPU mirrors.
 
 What it is for: kernels written after the round's GPU budget was spent (the Griffin-Lim glue kernels, the float16
@@ -8,59 +8,18 @@ hardware, doubles as the check that the emulator itself behaves.  It does not st
 ordering, real instruction behaviour, performance) -- those tests keep their `gpu` markers.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import data_oracle as DO
-from tacotron_b200 import _lib as L
 from tests import mirror_kernels as MK
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libtaco_emu.so")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_train.cpp", "emu_audio.cpp", "emu_data.cpp",
-                                                                 "emu_decoder_bwd.cpp", "emu_gru_bwd.cpp")]
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(ROOT, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_gemm.argtypes = [C.POINTER(L.GemmDesc), C.c_void_p]
-    lib.taco_last_error.restype = C.c_char_p
-    return lib
+from tests.emulator import KernelsOver, emu  # noqa: F401  (the emulated library, built once per process)
 
 
 def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
-
-
-class EmuK:
-    """the slice of tacotron_b200/kernels.py the emulated entry points cover, on CPU tensors"""
-    def __init__(self, lib):
-        self.lib = lib
-
-    def _ok(self, rc, what):
-        assert rc == 0, f"{what}: {self.lib.taco_last_error().decode()}"
-
-    def gemm(self, Cm, A, B, *, ta=False, tb=False, beta=0.0, shift=0, period=0, taps=1, dshift=0, kper=0, b_tap_stride=0,
-             batch=1, a_bstride=0, b_bstride=0, c_bstride=0, bshift=0):
-        M, N = Cm.shape
-        K = A.shape[0] if ta else A.shape[1] * taps
-        d = L.GemmDesc()
-        ld = lambda t: t.stride(0) if t.shape[0] > 1 else max(t.shape[1], t.stride(0))
-        d.A = A.data_ptr(); d.lda = ld(A); d.B = B.data_ptr(); d.ldb = ld(B); d.C = Cm.data_ptr(); d.ldc = ld(Cm)
-        d.M = M; d.N = N; d.K = K; d.ta = int(ta); d.tb = int(tb); d.beta = float(beta)
-        d.shift = shift; d.period = period; d.taps = taps; d.dshift = dshift; d.kper = kper; d.b_tap_stride = b_tap_stride
-        d.batch = batch; d.a_bstride = a_bstride; d.b_bstride = b_bstride; d.c_bstride = c_bstride; d.bshift = bshift
-        self._ok(self.lib.taco_gemm(C.byref(d), None), "taco_gemm")
 
 
 def _gemm_cases():
@@ -93,7 +52,7 @@ def _gemm_cases():
 @pytest.mark.parametrize("impl,tol", [(0, 2e-6), (1, 2e-5)])
 def test_gemm_kernels_under_emulation(emu, impl, tol):
     """impl 0 = the FFMA kernel (green on hardware: validates the emulator); impl 1 = the 3xTF32 mma.sync kernel"""
-    K = EmuK(emu)
+    K = KernelsOver(emu)
     prev = emu.taco_set_gemm_impl(impl)
     try:
         for name, Cs, As, Bs, cv, av, bv, kw in _gemm_cases():
@@ -139,7 +98,6 @@ def test_griffinlim_kernels_under_emulation(emu, r, T):
     reb[0, 0, :5] = 0
     p_c, p_e = torch.empty(B, n, F, dtype=torch.complex64), torch.empty(B, n, F, dtype=torch.complex64)
     MK.gl_phase(p_c, mag_c, reb)
-    emu.taco_gl_phase.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     assert emu.taco_gl_phase(_p(p_e), _p(mag_c), _p(reb), mag_c.numel(), None) == 0
     close(p_e, p_c, 1e-5)
 
@@ -165,20 +123,10 @@ def test_decoder_bwd_kernel_under_emulation(emu, r, sched):
         e[k].fill_(float("nan"))
     for i in range(3):
         e["DG"][i].fill_(float("nan")); e["DC"][i].fill_(float("nan"))
-    d = L.DecoderBwdArgs()
-    d.B, d.T, d.Tx, d.r, d.keep_scale = B, T, Tx, r, float(a["keep_scale"])
-    for k in ("W_a", "W_q", "W_out", "W_in", "W1", "W2", "v", "dy_ext", "align", "values", "keys", "PQ", "PN1", "PN2", "sel", *outs):
-        assert e[k].is_contiguous(), k
-        setattr(d, k, e[k].data_ptr())
     for k in ("Wg", "Wc", "RU", "C", "H", "DG", "DC"):
         for i in range(3):
             e[k][i] = e[k][i].contiguous()
-            getattr(d, k)[i] = e[k][i].data_ptr()
-    emu.taco_decoder_bwd_workspace_bytes.restype = C.c_size_t
-    ws = torch.empty(emu.taco_decoder_bwd_workspace_bytes() // 4)
-    d.workspace = ws.data_ptr()
-    emu.taco_decoder_bwd.argtypes = [C.POINTER(L.DecoderBwdArgs), C.c_void_p]
-    assert emu.taco_decoder_bwd(C.byref(d), None) == 0, emu.taco_last_error().decode()
+    KernelsOver(emu).decoder_bwd(e)
     for k in outs:
         got, ref = torch.nan_to_num(e[k], nan=1e30), a[k]
         assert (got - ref).abs().max().item() <= 2e-5 * (ref.abs().max().item() + 1e-6), k
@@ -193,8 +141,6 @@ def test_fft2048_kernels_under_emulation(emu):
     g = torch.Generator().manual_seed(11)
     x = torch.randn(3, 2048, generator=g)
     X = torch.empty(3, 1025, dtype=torch.complex64)
-    emu.taco_rfft2048.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
-    emu.taco_irfft2048.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     assert emu.taco_rfft2048(_p(X), _p(x), 3, None) == 0, emu.taco_last_error().decode()
     ref = torch.fft.rfft(x.double(), dim=-1)
     assert (X.to(torch.complex128) - ref).abs().max().item() <= 2e-6 * ref.abs().max().item()
@@ -220,13 +166,11 @@ def test_bigru_bwd_kernel_under_emulation(emu):
     ref = torch.zeros(B, T, 768)
     MK.bigru_bwd(ref, dOut, out, ACT, *W)
     got = torch.full((B, T, 768), float("nan"))
-    emu.taco_bigru_bwd.argtypes = [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_void_p]
     assert emu.taco_bigru_bwd(_p(got), _p(dOut), _p(out), _p(ACT), *[_p(w) for w in W], B, T, None) == 0
     assert (torch.nan_to_num(got, nan=1e30) - ref).abs().max().item() <= 2e-5 * ref.abs().max().item()
 
 
 def test_normalize_f16_under_emulation_is_bit_exact(emu):
-    emu.taco_normalize_f16.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]
     rng = np.random.RandomState(1)
     for shape in ((6, 5, 2050), (3, 7, 161), (1, 1, 161)):                          # even / odd widths and totals
         x = (rng.randn(*shape) * 3 - 2).astype(np.float16)

@@ -2,31 +2,12 @@
 mirror: the lane mapping, the select-free transposing butterflies and the 3-step prefetch rotation, checked without a
 GPU.  T = 1..4 and 7 cover every tail of the 3-step unrolled loop; B = 3 puts utterances at non-zero offsets."""
 import ctypes as C
-import os
-import subprocess
 
 import pytest
 import torch
 
 from tests import mirror_kernels_spk as MK
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu_bigru") / "libtaco_emu_bigru.so")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_gru.cpp")]
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(ROOT, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_bigru_fwd.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p]
-    lib.taco_bigru_fwd_h0.argtypes = [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_void_p]
-    return lib
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
 
 def _p(t):

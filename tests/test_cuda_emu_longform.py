@@ -2,8 +2,6 @@
 taco_speech_bounds against the float64 oracle and against taco_speech_frames, taco_join_segments against its float64
 mirror, and the argument checks of both.  Checks their indexing without a GPU."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -11,26 +9,7 @@ import torch
 
 from tests import longform_oracle as LO
 from tests import trim_oracle as TO
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
-
-
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu_longform") / "libtaco_emu_longform.so")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_audio.cpp")]
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(ROOT, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_speech_frames.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]
-    lib.taco_speech_bounds.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]
-    lib.taco_join_segments.argtypes = [vp, i64, vp, vp, i32, i32, i32, vp]
-    return lib
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
 
 def _p(t):

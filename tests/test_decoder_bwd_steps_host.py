@@ -3,16 +3,14 @@ kernel itself under the host emulation (tests/cuda_emu, the one-CTA build tests/
 mirror shows float64-level ratios, the emulated kernel passes, suffix runs compose bit for bit, one corrupted stored
 element is reported at exactly its (t, stage, b, unit), a fold rounded to TF32 is flagged where it is first used, and
 the bars of one small case match a hand restatement."""
-import ctypes as C
 import math
 
 import pytest
 import torch
 
-from tacotron_b200 import _lib as L
 from tests import decoder_bwd_step_checks as DB
 from tests import mirror_kernels_guided as MKG
-from tests.test_cuda_emu import emu  # noqa: F401  (the emulated library, built once per module)
+from tests.emulator import KernelsOver, emu  # noqa: F401  (the emulated library, built once per process)
 
 
 def _mirror(a):
@@ -21,36 +19,10 @@ def _mirror(a):
 
 def _emu_run(lib):
     """kernels.decoder_bwd over the emulated library, on CPU tensors (the workspace is kept in a['_ws'])"""
-    lib.taco_decoder_bwd_workspace_bytes.restype = C.c_size_t
-    lib.taco_decoder_bwd.argtypes = [C.POINTER(L.DecoderBwdArgs), C.c_void_p]
-
-    def run(a):
-        T, B, OUT = a["dy_ext"].shape
-        d = L.DecoderBwdArgs()
-        d.B, d.T, d.Tx, d.r, d.keep_scale = B, T, a["align"].shape[2], OUT // 80, float(a["keep_scale"])
-        for k in ("W_a", "W_q", "W_out", "W_in", "W1", "W2", "v", "dy_ext", "align", "values", "keys", "PQ", "PN1", "PN2",
-                  "sel", *DB.OUTS):
-            assert a[k].is_contiguous(), k
-            setattr(d, k, a[k].data_ptr())
-        for k in ("Wg", "Wc", "RU", "C", "H", "DG", "DC"):
-            for i in range(3):
-                getattr(d, k)[i] = a[k][i].data_ptr()
-        if a.get("H0") is not None:
-            for i in range(3):
-                d.H0[i] = a["H0"][i].data_ptr()
-        if a.get("DH0") is not None:
-            d.DH0 = a["DH0"].data_ptr()
-        if a.get("dscore_add") is not None:
-            d.dscore_add = a["dscore_add"].data_ptr()
-        ws = torch.empty(lib.taco_decoder_bwd_workspace_bytes() // 4)
-        d.workspace = ws.data_ptr()
-        assert lib.taco_decoder_bwd(C.byref(d), None) == 0, lib.taco_last_error().decode()
-        a["_ws"] = ws
-    return run
+    return KernelsOver(lib).decoder_bwd
 
 
 def test_workspace_layout(emu):  # noqa: F811
-    emu.taco_decoder_bwd_workspace_bytes.restype = C.c_size_t
     assert emu.taco_decoder_bwd_workspace_bytes() == DB.WS_TOTAL * 4
 
 

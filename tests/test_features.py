@@ -5,7 +5,6 @@ the host emulation."""
 import ctypes as C
 import os
 import pickle
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,6 +14,7 @@ from oracle import audio_oracle as A
 from tacotron_b200 import audio, preprocess as P
 from tests import feature_oracle as FO
 from tests import mirror_kernels_features as MKF
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_preprocess.npz")
@@ -197,25 +197,6 @@ def test_driver_over_mirrors(tmp_path):
 
 
 # ---- the kernel sources under the host emulation ----
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    out = str(tmp_path_factory.mktemp("emu_features") / "libtaco_emu_features.so")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_audio.cpp", "emu_features.cpp")]
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(ROOT, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_trim_bounds.argtypes = [vp, vp, vp, i32, i32, i32, f32, vp]
-    lib.taco_feature_frames.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
-    lib.taco_feature_spec.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
-    lib.taco_rfft2048.argtypes = [vp, vp, i64, vp]
-    return lib
-
-
 def _p(t):
     return C.c_void_p(t.data_ptr())
 

@@ -5,8 +5,6 @@ the training driver's command line."""
 import copy
 import ctypes as C
 import math
-import os
-import subprocess
 import types
 
 import pytest
@@ -17,8 +15,8 @@ from tacotron_b200 import _lib as L
 from tacotron_b200.models import grad
 from tacotron_b200.models.tacotron import Config, Tacotron
 from tests import grad_util, guided_attention_oracle as GA, mirror_kernels_guided as MKG, speaker_decoder_oracle as SD
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 G_PAPER = 0.2
 
 
@@ -133,27 +131,6 @@ def test_zero_lambda_gives_the_gradients_without_the_feature(spk):
 
 
 # ---- the kernel sources under the host emulation (tests/cuda_emu/emu.h) ----
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    root = os.path.dirname(HERE)
-    out = str(tmp_path_factory.mktemp("emu_ga") / "libtaco_emu_ga.so")
-    src = [os.path.join(root, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_train.cpp", "emu_decoder_bwd.cpp")]
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(root, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    vp, i32, f32 = C.c_void_p, C.c_int, C.c_float
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_gemm.argtypes = [C.POINTER(L.GemmDesc), vp]
-    lib.taco_decoder_bwd_workspace_bytes.restype = C.c_size_t
-    lib.taco_decoder_bwd.argtypes = [C.POINTER(L.DecoderBwdArgs), vp]
-    lib.taco_guided_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, vp, vp]
-    lib.taco_guided_attention_partial_count.argtypes = [i32, i32]
-    return lib
-
-
 def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 

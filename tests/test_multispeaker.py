@@ -3,7 +3,6 @@ against the reference's own model code, the TF name map, the hand-written backwa
 mirrors against torch.autograd, and the input pipeline's speaker ids."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,6 +14,7 @@ from tacotron_b200.models import grad
 from tacotron_b200.models.tacotron import Config
 from tacotron_b200.tf_names import tf_name_to_param
 from tests import grad_util_spk, mirror_kernels_spk as MK, speaker_oracle as SO
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 NSPK = 3
@@ -164,25 +164,6 @@ def test_device_batches_stage_speaker_ids():
 
 
 # ---- the new CUDA paths under the host emulation (tests/cuda_emu/emu.h): index algebra without a GPU ----
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    root = os.path.dirname(HERE)
-    out = str(tmp_path_factory.mktemp("emu_spk") / "libtaco_emu_spk.so")
-    src = [os.path.join(root, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_train.cpp", "emu_gru.cpp", "emu_gru_bwd.cpp")]
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(root, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_bigru_fwd.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p]
-    lib.taco_bigru_fwd_h0.argtypes = [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_void_p]
-    lib.taco_bigru_bwd_h0.argtypes = [C.c_void_p] * 11 + [C.c_int, C.c_int, C.c_void_p]
-    lib.taco_colsum_seg.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    return lib
-
-
 def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 

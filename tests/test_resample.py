@@ -5,7 +5,6 @@ emulation, and resampling inside process_audio_batch and the preprocessing drive
 import ctypes as C
 import os
 import pickle
-import subprocess
 from fractions import Fraction
 
 import numpy as np
@@ -17,8 +16,8 @@ from tests import feature_oracle as FO
 from tests import mirror_kernels_resample as MKR
 from tests import resample_oracle as RO
 from tests.test_features import _close_linear, _write_wav
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 RATES = [(48000, 24000), (44100, 16000), (22050, 16000), (48000, 16000), (16000, 24000), (8000, 16000)]
 
 
@@ -162,22 +161,6 @@ def test_too_short_to_resample_names_the_file(tmp_path):
 
 
 # ---- the kernel source under the host emulation ----
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    out = str(tmp_path_factory.mktemp("emu_resample") / "libtaco_emu_resample.so")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_resample.cpp")]
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(ROOT, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    vp, i32, i64 = C.c_void_p, C.c_int, C.c_int64
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_resample.argtypes = [vp, vp, vp, vp, i32, vp, i32, i32, C.c_double, vp, i64, vp]
-    return lib
-
-
 def _p(t):
     return C.c_void_p(t.data_ptr())
 

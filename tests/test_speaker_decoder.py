@@ -4,7 +4,6 @@ torch.autograd, the backward kernel's initial-state path under the host emulatio
 import copy
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -18,6 +17,7 @@ from tacotron_b200.models import grad
 from tacotron_b200.models.tacotron import Config
 from tacotron_b200.tf_names import tf_name_to_param
 from tests import mirror_kernels_spkdec as MK, speaker_decoder_oracle as SD, speaker_oracle as SO
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 NSPK = 3
@@ -129,24 +129,6 @@ def test_backward_matches_autograd(r, sched):
 
 
 # ---- the backward kernel's initial-state path under the host emulation (tests/cuda_emu/emu.h) ----
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    root = os.path.dirname(HERE)
-    out = str(tmp_path_factory.mktemp("emu_spkdec") / "libtaco_emu_spkdec.so")
-    src = [os.path.join(root, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_train.cpp", "emu_decoder_bwd.cpp")]
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(root, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_gemm.argtypes = [C.POINTER(L.GemmDesc), C.c_void_p]
-    lib.taco_decoder_bwd_workspace_bytes.restype = C.c_size_t
-    lib.taco_decoder_bwd.argtypes = [C.POINTER(L.DecoderBwdArgs), C.c_void_p]
-    return lib
-
-
 @pytest.mark.parametrize("r,sched", [(2, True), (5, False)])
 def test_decoder_bwd_kernel_with_h0_under_emulation(emu, r, sched):
     B, Tx, T = 2, 8, 4

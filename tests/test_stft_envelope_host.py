@@ -6,18 +6,12 @@ one batch past the 528-CTA grid and otherwise a handful of rows; every gl_ola / 
 smallest n.  Its sincospif / cospif are the float64 values rounded once (exact
 at multiples of 1/2, as on the device), so the same bars hold with more margin.
 """
-import ctypes as C
-import os
-import subprocess
-
 import pytest
 import torch
 
 from tacotron_b200 import audio
 from tests import stft_envelope_checks as SE
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
+from tests.emulator import KernelsOver, emu  # noqa: F401  (the emulated library, built once per process)
 
 # (B, n, hop, n_fft, win_length): production at the smallest n gl_frame takes and at n = 2 (gl_ola only), win = n_fft,
 # odd n_fft - win, hop not dividing win, hop in (win/2, win], hop = win, hop > win, the smallest L gl_frame takes
@@ -29,33 +23,8 @@ OLA_FRAME = [(2, 5, 300, 2048, 1200), (3, 2, 300, 2048, 1200), (1, 9, 300, 2048,
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    out = str(tmp_path_factory.mktemp("emu_stft_env") / "libtaco_emu_stft_env.so")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_audio.cpp", "emu_features.cpp")]
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I",
-                           os.path.join(ROOT, "include"), *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_gl_init.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]      # as tacotron_b200/_lib.py
-    lib.taco_gl_ola.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]
-    lib.taco_gl_frame.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp]
-    lib.taco_gl_phase.argtypes = [vp, vp, vp, i64, vp]
-    lib.taco_rfft2048.argtypes = [vp, vp, i64, vp]
-    lib.taco_irfft2048.argtypes = [vp, vp, i64, vp]
-    lib.taco_gl_init_packed.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
-    lib.taco_gl_ola_packed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
-    lib.taco_gl_frame_packed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
-    lib.taco_feature_frames.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
-    lib.taco_feature_spec.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
-    return lib
-
-
-@pytest.fixture(scope="module")
-def env(lib):
-    return SE.Env(SE.LibK(lib), lib, "cpu")
+def env(emu):  # noqa: F811
+    return SE.Env(KernelsOver(emu), emu, "cpu")
 
 
 def test_fft_forward_classes(env):

@@ -6,7 +6,6 @@ import ctypes as C
 import math
 import os
 import struct
-import subprocess
 import sys
 import zlib
 
@@ -17,8 +16,8 @@ import torch
 from tacotron_b200 import summary as S
 from tests import mirror_kernels_summary as MKS
 from tests import summary_oracle as SO
+from tests.emulator import emu  # noqa: F401  (the emulated library, built once per process)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NLIM = 1551
 FLT_MAX = float(np.finfo(np.float32).max)
 
@@ -143,23 +142,6 @@ def test_mirror_all_nonfinite():
 
 
 # ---- the kernel source under the host emulation ----
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    out = str(tmp_path_factory.mktemp("emu_summary") / "libtaco_emu_summary.so")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_summary.cpp")]
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I", os.path.join(ROOT, "include"),
-                           *src, "-o", out])
-    lib = C.CDLL(out)
-    vp, i32, i64 = C.c_void_p, C.c_int, C.c_int64
-    lib.taco_last_error.restype = C.c_char_p
-    lib.taco_histogram_workspace_bytes.restype = C.c_size_t
-    lib.taco_histogram.argtypes = [vp, i64, vp, i32, vp, vp, vp, vp, vp]
-    return lib
-
-
 def _emu_run(emu, x):
     """the entry point with host pointers, NaN-poisoned workspace and outputs -> res int64 [nlim + 5]"""
     xt = torch.from_numpy(np.asarray(x, dtype=np.float32).copy())

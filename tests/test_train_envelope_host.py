@@ -14,84 +14,16 @@ boundaries, and every kernel of csrc/train.cu under the host emulation (tests/cu
   (whose fixed grid wraps from 303,104 elements) wrap here; bias_act, mul_shift, epi_bwd, epi_fwd_keep, maxpool_bwd,
   highway_fwd / bwd, l1_bwd, scatter_add_rows, dec_inputs and adam_step wrap only in tests/test_gpu_train_envelope.py.
 """
-import ctypes as C
-import os
-import subprocess
-from contextlib import ExitStack
-from unittest import mock
-
 import pytest
 import torch
 
 from oracle import tacotron_oracle as O
-from tacotron_b200 import _lib as L
 from tacotron_b200 import kernels
 from tacotron_b200.models import grad
 from tests import grad_util, grad_util_spk, mirror_kernels_spkdec as MKD, speaker_decoder_oracle as SD, speaker_oracle as SO
 from tests import train_envelope_cases as TE
 from tests import train_envelope_checks as CH
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-vp, i64, i32, f32 = C.c_void_p, C.c_int64, C.c_int, C.c_float
-ARGTYPES = {                                     # as tacotron_b200/_lib.py declares them
-    "taco_gemm": [C.POINTER(L.GemmDesc), vp],
-    "taco_colsum": [vp, vp, i64, vp, i64, vp, i64, i32, i32, vp],
-    "taco_colsum_seg": [vp, i64, vp, i64, i32, i32, i32, vp],
-    "taco_bias_act": [vp, i64, i32, i32, vp, i32, vp],
-    "taco_mul_shift": [vp, i64, vp, i64, vp, i64, i32, i32, i32, i32, vp],
-    "taco_epi_bwd": [vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, i32, vp, vp, f32, vp],
-    "taco_epi_fwd_keep": [vp, i64, vp, i32, i32, f32, vp],
-    "taco_bn_param_grad": [vp, vp, vp, vp, vp, vp, i32, vp],
-    "taco_maxpool_bwd": [vp, vp, vp, i32, i32, i32, vp],
-    "taco_highway_fwd": [vp, i64, vp, i64, vp, i64, i32, i32, vp],
-    "taco_highway_bwd": [vp, i64, vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, vp],
-    "taco_l1_bwd": [vp, vp, vp, i64, f32, vp],
-    "taco_l1_bwd_ld": [vp, i64, vp, vp, i64, i64, f32, vp],
-    "taco_scatter_add_rows": [vp, vp, vp, i32, i32, i32, vp],
-    "taco_dec_inputs": [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp],
-    "taco_attn_bwd_post": [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp],
-    "taco_sumsq": [vp, i64, vp, vp, vp],
-    "taco_adam_step": [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp, vp],
-}
-
-
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu_train") / "libtaco_emu_train.so")
-    cuda_inc = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("CUDA toolkit headers not found")
-    src = [os.path.join(ROOT, "tests", "cuda_emu", f) for f in ("emu_lib.cpp", "emu_train.cpp")]
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-I", cuda_inc, "-I",
-                           os.path.join(ROOT, "include"), *src, "-o", out])
-    lib = C.CDLL(out)
-    lib.taco_last_error.restype = C.c_char_p
-    for name, a in ARGTYPES.items():
-        getattr(lib, name).argtypes = a
-    return lib
-
-
-class EmuK:
-    """tacotron_b200.kernels over the emulated library: the product's own marshalling, with host pointers"""
-
-    def __init__(self, lib):
-        self.lib = lib
-
-    def __getattr__(self, name):
-        f = getattr(kernels, name)
-
-        def call(*a, **kw):
-            with ExitStack() as st:
-                st.enter_context(mock.patch.object(L, "lib", lambda: self.lib))
-                st.enter_context(mock.patch.object(kernels, "_st", lambda: None))
-                st.enter_context(mock.patch.object(kernels, "_chk2", lambda t, name: t))
-                return f(*a, **kw)
-        return call
-
-    def adam_step(self, p, g, m, v, lr_t, b1, b2, eps, clip, sumsq_t):       # kernels.adam_step insists on CUDA tensors
-        P = lambda t: C.c_void_p(t.data_ptr())
-        rc = self.lib.taco_adam_step(P(p), P(g), P(m), P(v), p.numel(), lr_t, b1, b2, eps, clip, P(sumsq_t), None)
-        assert rc == 0, self.lib.taco_last_error().decode()
+from tests.emulator import KernelsOver, emu  # noqa: F401  (the emulated library, built once per process)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -211,7 +143,7 @@ def test_gemm_envelope_under_emulation(emu, impl):
 
 
 def test_elementwise_kernels_under_emulation(emu):
-    K = EmuK(emu)
+    K = KernelsOver(emu)
     for act in (kernels.ACT_NONE, kernels.ACT_RELU):
         CH.check_bias_act(K, "cpu", "tiny", act, "exact")
     for act in (kernels.ACT_SIGMOID, kernels.ACT_TANH):
@@ -243,7 +175,7 @@ def test_elementwise_kernels_under_emulation(emu):
 def test_shaped_kernels_under_emulation(emu):
     """multi-row shapes the tiny edges do not reach: shifts inside several period blocks, maxpool ties across rows,
     colsum over several row blocks, attention over several steps, the 1028-pitch gradient over many rows"""
-    K = EmuK(emu)
+    K = KernelsOver(emu)
     g = torch.Generator().manual_seed(0)
     CH.check_maxpool_bwd(K, "cpu", "tiny")
     sizes = {"mp": (2, 9, 128)}
@@ -272,6 +204,6 @@ def test_shaped_kernels_under_emulation(emu):
 def test_grid_stride_wrap_under_emulation(emu):
     """two launches whose grid wraps: l1_bwd_ld over the [rows][1025] gradient in its 1028 pitch, sumsq over its fixed
     1184-block grid (303,104 threads) -- run once each"""
-    K = EmuK(emu)
+    K = KernelsOver(emu)
     CH.check_l1_bwd(K, "cpu", "wrap", 1.0, padded=True)
     CH.check_sumsq(K, "cpu", 1184 * 256 + 777, repeat=False)
