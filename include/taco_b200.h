@@ -416,6 +416,18 @@ int taco_gl_ola(float* y, const float* fr, int B, int n, int hop, int n_fft, int
 int taco_gl_frame(float* frw, const float* y, int B, int n, int hop, int n_fft, int win_length, void* stream);
 /* full = mag * rebuilt/|rebuilt|  (audio.py:84,87) over `count` complex elements */
 int taco_gl_phase(float* full_c64, const float* mag, const float* rebuilt_c64, int64_t count, void* stream);
+/* fast Griffin-Lim's phase update (Perraudin, Balazs & Sondergaard 2013; librosa >= 0.7's griffinlim):
+ * full = mag * d/|d|, d = rebuilt - beta*prev, and mag + 0i where d == 0 (as taco_gl_phase does for rebuilt == 0), over
+ * `count` complex elements.  prev is the previous iteration's rebuilt spectrum, beta = momentum / (1 + momentum) in
+ * [0, 0.5]; beta = 0 gives taco_gl_phase's values.  Element-wise, so the padded and packed layouts both use it.     */
+int taco_gl_phase_momentum(float* full_c64, const float* mag, const float* rebuilt_c64, const float* prev_c64, float beta,
+                           int64_t count, void* stream);
+/* De-emphasis, the inverse of preprocessing's pre-emphasis y[n] - coef*y[n-1]: in place, for each segment s in [0, S),
+ * y[i] = x[i] + coef*y[i-1] for i in [start[s], start[s+1]) with zero state before start[s]
+ * (scipy.signal.lfilter([1], [1, -coef], x) per segment).  start: device int64 [S+1], non-decreasing (the caller checks
+ * it); segments may be empty, nothing at or past start[S] is read.  One launch, one CTA per segment walking it in tiles
+ * with a block scan of the recurrence; deterministic.  S >= 0, 0 <= coef < 1.                                        */
+int taco_de_emphasis(float* y, const int64_t* start, int S, float coef, void* stream);
 /* the two transforms of a Griffin-Lim iteration (librosa.istft / librosa.stft inside audio.griffinlim, audio.py:84-86),
  * n_fft = 2048: X [rows][1025] complex (interleaved re, im) <-> x [rows][2048] real.  rfft is unnormalised, irfft scales
  * by 1/2048 and ignores the imaginary parts of the DC and Nyquist bins (numpy / cuFFT conventions).  Shared-memory

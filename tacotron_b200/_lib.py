@@ -182,6 +182,9 @@ SIGNATURES = {
     # where speech starts and ends, and the join of synthesised pieces (long-form synthesis)
     "taco_speech_bounds": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, f32, vp]),
     "taco_join_segments": (i32, [vp, i64, vp, vp, i32, i32, i32, vp]),
+    # fast Griffin-Lim and de-emphasis (opt-in synthesis options)
+    "taco_gl_phase_momentum": (i32, [vp, vp, vp, vp, f32, i64, vp]),
+    "taco_de_emphasis": (i32, [vp, vp, i32, f32, vp]),
     # input data format
     "taco_normalize_f16": (i32, [vp, vp, vp, vp, i64, i32, vp]),
     # feature extraction (preprocessing)

@@ -16,6 +16,8 @@ so one iteration is irfft2048 -> gl_ola -> gl_frame -> rfft2048 -> gl_phase: 5 l
 orchestration over tests/mirror_kernels.py on CPU tensors against the numpy oracle (oracle/audio_oracle.py).
 ``speech_frames`` / ``invert_speech`` are the opt-in tail trim of synthesis: where each utterance's speech ends
 (taco_speech_frames), then the same loop over only the kept frames of the batch, packed end to end.
+``momentum`` (every inversion entry point) is fast Griffin-Lim: gl_phase_momentum in place of gl_phase, with two rebuilt
+buffers written in turn.  ``de_emphasis`` undoes preprocessing's pre-emphasis on synthesised waveforms (taco_de_emphasis).
 
 Feature extraction (the reference's ``process_audio``, audio.py:38-65, used by tacotron_b200/preprocess.py) is the
 analysis half of the same transform: trim_bounds -> feature_frames -> rfft2048 -> feature_spec, four launches per chunk of
@@ -313,11 +315,13 @@ def reshape_frames(signal, r, forward=False):
     return s.permute(0, 2, 1, 3).reshape(nb * 4 * r, Fd)                     # frame = 4r*b + 4c + tl
 
 
-def griffinlim_batch(spec, r, n_iter=50, scale=None, shift=None, phase_u=None, K=None, generator=None):
+def griffinlim_batch(spec, r, n_iter=50, scale=None, shift=None, phase_u=None, K=None, generator=None, momentum=0.0):
     """spec [B, T, 1025*r] (log magnitudes in the decoder's r-frames-per-step layout, optionally normalised:
     magnitude = exp(spec*scale + shift), the driver's ``out*stft_std + stft_mean`` of test.py:64) -> waveforms [B, L],
-    L = hop*(4r*(T//4) - 1).  phase_u: uniform [0,1) initial phases [B, n, 1025] (audio.py:81), drawn if None."""
+    L = hop*(4r*(T//4) - 1).  phase_u: uniform [0,1) initial phases [B, n, 1025] (audio.py:81), drawn if None.
+    momentum in [0, 1]: fast Griffin-Lim (_gl_iterations); 0 is the reference's plain loop."""
     K = K or _K()
+    gl_check(n_iter, momentum)
     B, T, W = spec.shape
     assert W == F_BINS * r, (W, r)
     n = 4 * r * (T // 4)
@@ -332,15 +336,36 @@ def griffinlim_batch(spec, r, n_iter=50, scale=None, shift=None, phase_u=None, K
     full = torch.empty((B, n, F_BINS), dtype=cdt, device=spec.device)
     y = torch.empty((B, L), dtype=rdt, device=spec.device)
     frw = torch.empty((B, n, n_fft), dtype=rdt, device=spec.device)
-    _gl_iterations(K, full, mag, spec, phase_u, r, scale, shift, y, frw, n_iter)
+    _gl_iterations(K, full, mag, spec, phase_u, r, scale, shift, y, frw, n_iter, momentum=momentum)
     return y
 
 
-def _gl_iterations(K, full, mag, spec, phase_u, r, scale, shift, y, frw, n_iter, rebuilt=None, packed=None):
+def gl_check(n_iter, momentum):
+    """n_iter an integer >= 0 and momentum a number in [0, 1], else ValueError naming the value; -> beta =
+    momentum / (1 + momentum), the weight of the previous iterate in fast Griffin-Lim's update"""
+    if isinstance(n_iter, bool) or not isinstance(n_iter, (int, np.integer)) or n_iter < 0:
+        raise ValueError(f"Griffin-Lim: n_iter = {n_iter!r} must be an integer >= 0")
+    try:
+        m = float(momentum)
+    except (TypeError, ValueError):
+        m = float("nan")
+    if isinstance(momentum, bool) or not 0.0 <= m <= 1.0:
+        raise ValueError(f"Griffin-Lim: momentum = {momentum!r} must be a number in [0, 1]")
+    return m / (1.0 + m)
+
+
+def _gl_iterations(K, full, mag, spec, phase_u, r, scale, shift, y, frw, n_iter, rebuilt=None, packed=None, momentum=0.0):
     """frw [B, n, 2048] doubles as the istft frame buffer: irfft writes it, gl_ola consumes it, gl_frame refills it.
-    packed: (off, max_frames) of invert_speech's packed layout (rows off[b]:off[b+1] per utterance), None for [B, n, .]."""
+    packed: (off, max_frames) of invert_speech's packed layout (rows off[b]:off[b+1] per utterance), None for [B, n, .].
+    momentum > 0: fast Griffin-Lim (Perraudin, Balazs & Sondergaard 2013; librosa >= 0.7), angles = d/|d| with
+    d = rebuilt - beta*rebuilt_prev, beta = momentum/(1 + momentum).  rebuilt: one buffer like full, or the two the FFT
+    writes in turn when momentum > 0 (the other holds the previous iterate, so nothing is copied).  momentum = 0 is the
+    plain loop, launch for launch."""
+    beta = gl_check(n_iter, momentum)
     if rebuilt is None:
-        rebuilt = torch.empty_like(full)
+        rebuilt = torch.empty_like(full) if beta == 0 else (torch.empty_like(full), torch.empty_like(full))
+    elif beta > 0 and not isinstance(rebuilt, tuple):
+        raise ValueError("Griffin-Lim with momentum needs two rebuilt buffers")
     if packed is None:
         K.gl_init(full, mag, spec, phase_u, r, scale, shift)
         ola = functools.partial(K.gl_ola, y, frw, hop_length, win_length)
@@ -356,8 +381,16 @@ def _gl_iterations(K, full, mag, spec, phase_u, r, scale, shift, y, frw, n_iter,
         if it == n_iter:
             break
         frame()
-        K.rfft2048(rebuilt, frw)                                             # real FFT of every re-framed, windowed frame
-        K.gl_phase(full, mag, rebuilt)
+        if beta == 0:
+            K.rfft2048(rebuilt, frw)                                         # real FFT of every re-framed, windowed frame
+            K.gl_phase(full, mag, rebuilt)
+            continue
+        cur, prev = rebuilt[it % 2], rebuilt[(it + 1) % 2]
+        K.rfft2048(cur, frw)
+        if it == 0:                                                          # rebuilt_prev = 0
+            K.gl_phase(full, mag, cur)
+        else:
+            K.gl_phase_momentum(full, mag, cur, prev, beta)
 
 
 def speech_frames(spec, r, stft_mean=None, stft_std=None, top_db=TRIM_TOP_DB, K=None):
@@ -387,20 +420,23 @@ def stop_frames(end_step, r, T, frames=None):
     return f.to(torch.int32)
 
 
-def invert_speech(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, generator=None):
+def invert_speech(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, generator=None,
+                  momentum=0.0):
     """invert_spectrogram on the first frames[b] STFT frames of each utterance only (frames: speech_frames or the
     caller's, a multiple of 4r in [5, 4r*(T//4)] each) -> list of B 1-D waveforms of hop*(frames[b]-1) samples.  The kept
     frames are packed end to end, so one iteration is still 5 launches; utterance b equals invert_spectrogram on
     spec[b:b+1, :frames[b]//r] with the same initial phases.  phase_u: packed uniform [0,1) phases [sum(frames), 1025],
     drawn on the device if None.  Reads frames to the host once."""
-    y, start = invert_speech_packed(spec, r, frames, n_iter, stft_mean, stft_std, phase_u, K, generator)
+    y, start = invert_speech_packed(spec, r, frames, n_iter, stft_mean, stft_std, phase_u, K, generator, momentum)
     return [y[start[b]:start[b + 1]] for b in range(len(start) - 1)]
 
 
-def invert_speech_packed(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, generator=None):
+def invert_speech_packed(spec, r, frames, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, generator=None,
+                         momentum=0.0):
     """invert_speech's waveforms as the one flat buffer Griffin-Lim writes: (y, start) with utterance b in
     y[start[b]:start[b+1]] (start int64 numpy [B+1])"""
     K = K or _K()
+    gl_check(n_iter, momentum)
     B, T, W = spec.shape
     assert W == F_BINS * r, (W, r)
     n = 4 * r * (T // 4)
@@ -426,7 +462,7 @@ def invert_speech_packed(spec, r, frames, n_iter=50, stft_mean=None, stft_std=No
     y = torch.empty(hop_length * (N - B), dtype=rdt, device=dev)
     frw = torch.empty((N, n_fft), dtype=rdt, device=dev)
     _gl_iterations(K, full, mag, spec.contiguous(), phase_u.contiguous(), r, scale, shift, y, frw, n_iter,
-                   packed=(torch.from_numpy(off).to(dev), nmax))
+                   packed=(torch.from_numpy(off).to(dev), nmax), momentum=momentum)
     return y, hop_length * (off - np.arange(B + 1))
 
 
@@ -463,11 +499,13 @@ class GriffinLimGraph:
     """The same 5-launches-per-iteration loop captured ONCE into a CUDA graph for a fixed (B, T, r, n_iter) and replayed:
     251 launches (and their Python / ctypes overhead, ~0.1 ms per iteration of host time) collapse into one
     graph launch.  Inputs are copied into static device buffers; the result is the static `y` (valid until the next call).
-    Opt-in: `invert_spectrogram(...)` stays eager."""
+    Opt-in: `invert_spectrogram(...)` stays eager.  momentum > 0: fast Griffin-Lim, with the second rebuilt buffer among
+    the static ones."""
 
-    def __init__(self, B, T, r, n_iter=50, device="cuda", with_affine=True):
+    def __init__(self, B, T, r, n_iter=50, device="cuda", with_affine=True, momentum=0.0):
         K = _K()
-        self.B, self.T, self.r, self.n_iter = B, T, r, n_iter
+        beta = gl_check(n_iter, momentum)
+        self.B, self.T, self.r, self.n_iter, self.momentum = B, T, r, n_iter, momentum
         n = 4 * r * (T // 4)
         L = hop_length * (n - 1)
         assert L > n_fft // 2
@@ -481,17 +519,17 @@ class GriffinLimGraph:
         self.full = torch.empty((B, n, F_BINS), dtype=torch.complex64, device=dev)
         self.y = torch.empty((B, L), **f32)
         self.frw = torch.empty((B, n, n_fft), **f32)
-        self.rebuilt = torch.empty_like(self.full)
+        self.rebuilt = torch.empty_like(self.full) if beta == 0 else (torch.empty_like(self.full), torch.empty_like(self.full))
         args = (K, self.full, self.mag, self.spec, self.phase_u, r, self.scale, self.shift, self.y, self.frw, n_iter, self.rebuilt)
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                     # warm-up outside capture: lazy module loads
-            _gl_iterations(*args)
+            _gl_iterations(*args, momentum=momentum)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            _gl_iterations(*args)
+            _gl_iterations(*args, momentum=momentum)
 
     def __call__(self, spec, stft_mean=None, stft_std=None, phase_u=None, generator=None):
         self.spec.copy_(spec.reshape(self.spec.shape), non_blocking=True)
@@ -508,7 +546,7 @@ class GriffinLimGraph:
         return self.y
 
 
-def griffinlim(spectrogram, n_iter=50, phase_u=None, K=None):
+def griffinlim(spectrogram, n_iter=50, phase_u=None, K=None, momentum=0.0):
     """audio.griffinlim for ONE magnitude spectrogram [1025, frames] (audio.py:77) -> waveform [hop*(frames-1)]."""
     Fd, n = spectrogram.shape
     assert Fd == F_BINS
@@ -516,16 +554,33 @@ def griffinlim(spectrogram, n_iter=50, phase_u=None, K=None):
     # r=1: reshape_frames(forward=False) is the identity on whole blocks of 4 frames
     assert n % 4 == 0, "frame count must be a multiple of 4 (the reference always produces 4r-frame blocks)"
     pu = None if phase_u is None else phase_u[None]
-    return griffinlim_batch(spec, 1, n_iter=n_iter, phase_u=pu, K=K)[0]
+    return griffinlim_batch(spec, 1, n_iter=n_iter, phase_u=pu, K=K, momentum=momentum)[0]
 
 
-def invert_spectrogram(spec, r, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None):
+def invert_spectrogram(spec, r, n_iter=50, stft_mean=None, stft_std=None, phase_u=None, K=None, momentum=0.0):
     """audio.invert_spectrogram (audio.py:67-75) with the driver's de-normalisation folded in.
-    spec [T, 1025*r] or [B, T, 1025*r] on the device -> waveform(s)."""
+    spec [T, 1025*r] or [B, T, 1025*r] on the device -> waveform(s).  momentum: fast Griffin-Lim (griffinlim_batch)."""
     single = spec.dim() == 2
     s = spec[None] if single else spec
     scale, shift = (stft_std, stft_mean) if stft_std is not None else (None, None)
     if phase_u is not None and single:
         phase_u = phase_u[None]
-    y = griffinlim_batch(s.contiguous(), r, n_iter=n_iter, scale=scale, shift=shift, phase_u=phase_u, K=K)
+    y = griffinlim_batch(s.contiguous(), r, n_iter=n_iter, scale=scale, shift=shift, phase_u=phase_u, K=K, momentum=momentum)
     return y[0] if single else y
+
+
+def de_emphasis(y, start=None, K=None):
+    """Undo preprocessing's pre-emphasis (PRE_EMPHASIS, audio.py:53) on synthesised waveforms, in place: y[i] = x[i] +
+    PRE_EMPHASIS*y[i-1] over each segment [start[s], start[s+1]) of y, zero state before start[s] (scipy.signal.lfilter
+    ([1], [1, -PRE_EMPHASIS], .) per segment).  y: contiguous fp32 on the device.  start (host int64 [S+1]): None for the
+    rows of a [B, L] y, else e.g. invert_speech_packed's start or the spans of long-form lines.  One launch; no host
+    synchronisation.  Returns y."""
+    K = K or _K()
+    if start is None:
+        if y.dim() != 2:
+            raise ValueError(f"de_emphasis: without start, y must be [B, L], got {tuple(y.shape)}")
+        start = np.arange(y.shape[0] + 1, dtype=np.int64) * y.shape[1]
+    elif torch.is_tensor(start):
+        start = start.cpu().numpy()
+    K.de_emphasis(y, start, PRE_EMPHASIS)
+    return y

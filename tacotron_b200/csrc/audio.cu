@@ -127,6 +127,114 @@ __global__ void gl_phase_kernel(float2* __restrict__ full, const float* __restri
     }
 }
 
+// fast Griffin-Lim's phase update: full = mag * d/|d|, d = rebuilt - beta * prev (angle(0) = 0 -> unit phasor 1).
+// gl_phase's arithmetic on d, so beta = 0 gives gl_phase's values.
+__global__ void gl_phase_momentum_kernel(float2* __restrict__ full, const float* __restrict__ mag, const float2* __restrict__ rebuilt,
+                                         const float2* __restrict__ prev, float beta, int64_t total) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const float2 z = rebuilt[i], p = prev[i];
+        const float2 d = make_float2(fmaf(-beta, p.x, z.x), fmaf(-beta, p.y, z.y));
+        const float a = hypotf(d.x, d.y);
+        const float m = mag[i];
+        full[i] = (a > 0.f) ? make_float2(m * (d.x / a), m * (d.y / a)) : make_float2(m, 0.f);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// De-emphasis of synthesised waveforms (taco_de_emphasis): y[i] = x[i] + c y[i-1] in place over each segment
+// [start[s], start[s+1]), zero state before start[s].  One CTA per segment walks it in tiles of DE_TILE samples, carrying
+// the last output of a tile into the next; no CTA waits on another.  Within a tile:
+//   - the tile is staged in shared memory (coalesced; one pad word per DE_ITEMS samples keeps the per-thread reads
+//     conflict-free) while the next tile's loads are already in flight in registers;
+//   - thread t runs the recurrence over its DE_ITEMS consecutive samples from zero state: loc[i], and the affine map
+//     y_in -> c^len y_in + loc[len-1] its run applies to the state it receives;
+//   - a block scan composes those maps in order (warp shuffles, then the warp totals serially), so thread t learns the
+//     state y_in before its first sample from the carry; it writes loc[i] + c^(i+1) y_in.
+// Every reduction has a fixed order: the same bits every run.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int DE_THREADS = 512, DE_ITEMS = 16, DE_TILE = DE_THREADS * DE_ITEMS;
+constexpr int DE_WARPS = DE_THREADS / 32;
+
+__device__ __forceinline__ int de_slot(int e) { return e + e / DE_ITEMS; }
+
+__global__ void __launch_bounds__(DE_THREADS) de_emphasis_kernel(float* __restrict__ y, const int64_t* __restrict__ start, float c) {
+    __shared__ float sm[DE_TILE + DE_TILE / DE_ITEMS];
+    __shared__ float wa[DE_WARPS], wb[DE_WARPS];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t s0 = start[blockIdx.x], s1 = start[blockIdx.x + 1];
+    float v[DE_ITEMS];
+#pragma unroll
+    for (int j = 0; j < DE_ITEMS; ++j) {
+        const int64_t g = s0 + j * DE_THREADS + tid;
+        v[j] = g < s1 ? y[g] : 0.f;
+    }
+    float carry = 0.f;                                                  // the output just before the tile
+    for (int64_t t0 = s0; t0 < s1; t0 += DE_TILE) {
+        const int len = (int)(s1 - t0 < DE_TILE ? s1 - t0 : DE_TILE);
+#pragma unroll
+        for (int j = 0; j < DE_ITEMS; ++j) sm[de_slot(j * DE_THREADS + tid)] = v[j];
+        __syncthreads();
+        const int64_t t1 = t0 + DE_TILE;                                // prefetch the next tile
+#pragma unroll
+        for (int j = 0; j < DE_ITEMS; ++j) {
+            const int64_t g = t1 + j * DE_THREADS + tid;
+            v[j] = g < s1 ? y[g] : 0.f;
+        }
+        int mine = len - tid * DE_ITEMS;                                // samples of this thread in the tile
+        mine = mine < 0 ? 0 : (mine > DE_ITEMS ? DE_ITEMS : mine);
+        const float* xs = sm + tid * (DE_ITEMS + 1);                    // = sm + de_slot(tid * DE_ITEMS)
+        float loc[DE_ITEMS];
+        float acc = 0.f, a = 1.f;
+#pragma unroll
+        for (int i = 0; i < DE_ITEMS; ++i) {
+            if (i < mine) {
+                acc = fmaf(c, acc, xs[i]);
+                a *= c;
+            }
+            loc[i] = acc;
+        }
+        // This run's map is y_in -> a y_in + b.  Butterfly scan of the maps over the warp: at step m, (a, b) is the
+        // composition of this lane's aligned block of m lanes, and (ea, eb) that of the lanes before it in the block; the
+        // partner block (lane ^ m) is composed in front when it comes first, behind otherwise.  Both halves spell the
+        // composition with the same operands, so every lane ends with the same warp total.
+        float b = acc, ea = 1.f, eb = 0.f;
+#pragma unroll
+        for (int m = 1; m < 32; m <<= 1) {
+            const float oa = __shfl_xor_sync(0xffffffffu, a, m), ob = __shfl_xor_sync(0xffffffffu, b, m);
+            if (lane & m) {                                             // partner block first: (oa, ob) then ours
+                eb = fmaf(ea, ob, eb);
+                ea *= oa;
+                b = fmaf(a, ob, b);
+            } else {                                                    // ours first, then the partner's
+                b = fmaf(oa, b, ob);
+            }
+            a *= oa;
+        }
+        if (lane == 31) { wa[warp] = a; wb[warp] = b; }
+        __syncthreads();
+        float yw = carry;                                               // the state entering this warp's first lane
+        for (int w = 0; w < warp; ++w) yw = fmaf(wa[w], yw, wb[w]);
+        const float yin = fmaf(ea, yw, eb);
+        float* ys = sm + tid * (DE_ITEMS + 1);
+        float p = 1.f;
+#pragma unroll
+        for (int i = 0; i < DE_ITEMS; ++i) {
+            if (i < mine) {
+                p *= c;
+                ys[i] = fmaf(p, yin, loc[i]);
+            }
+        }
+        __syncthreads();
+        carry = sm[de_slot(len - 1)];
+#pragma unroll
+        for (int j = 0; j < DE_ITEMS; ++j) {
+            const int e = j * DE_THREADS + tid;
+            if (e < len) y[t0 + e] = sm[de_slot(e)];
+        }
+        __syncthreads();                                                // sm, wa and wb are rewritten by the next tile
+    }
+}
+
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Where an utterance's speech ends (taco_speech_frames).  Two launches: frame_power_kernel spreads the read of the
@@ -558,6 +666,27 @@ int taco_gl_phase(float* full_c64, const float* mag, const float* rebuilt_c64, i
     if (count == 0) return 0;
     TACO_LAUNCH(gl_phase_kernel, grid_for(count, 256), 256, 0, (cudaStream_t)stream, reinterpret_cast<float2*>(full_c64), mag,
                                                                             reinterpret_cast<const float2*>(rebuilt_c64), count);
+    TACO_LAUNCH_CHECK();
+    return 0;
+}
+
+int taco_gl_phase_momentum(float* full_c64, const float* mag, const float* rebuilt_c64, const float* prev_c64, float beta,
+                           int64_t count, void* stream) {
+    TACO_CHECK(full_c64 && mag && rebuilt_c64 && prev_c64 && count >= 0, "taco_gl_phase_momentum: bad arguments");
+    TACO_CHECK(beta >= 0.f && beta <= 0.5f, "taco_gl_phase_momentum: beta=%g outside [0, 0.5]", (double)beta);
+    if (count == 0) return 0;
+    TACO_LAUNCH(gl_phase_momentum_kernel, grid_for(count, 256), 256, 0, (cudaStream_t)stream, reinterpret_cast<float2*>(full_c64),
+                mag, reinterpret_cast<const float2*>(rebuilt_c64), reinterpret_cast<const float2*>(prev_c64), beta, count);
+    TACO_LAUNCH_CHECK();
+    return 0;
+}
+
+int taco_de_emphasis(float* y, const int64_t* start, int S, float coef, void* stream) {
+    TACO_CHECK(y && start, "taco_de_emphasis: NULL");
+    TACO_CHECK(S >= 0, "taco_de_emphasis: S=%d segments", S);
+    TACO_CHECK(coef >= 0.f && coef < 1.f, "taco_de_emphasis: coef=%g outside [0, 1)", (double)coef);
+    if (S == 0) return 0;
+    TACO_LAUNCH(de_emphasis_kernel, S, DE_THREADS, 0, (cudaStream_t)stream, y, start, coef);
     TACO_LAUNCH_CHECK();
     return 0;
 }

@@ -427,6 +427,46 @@ def gl_phase(full, mag, rebuilt):
     L.check(L.lib().taco_gl_phase(_p(full), _p(mag), _p(rebuilt), mag.numel(), _st()), "taco_gl_phase")
 
 
+def gl_phase_momentum(full, mag, rebuilt, prev, beta):
+    """full = mag * d/|d|, d = rebuilt - beta*prev (mag + 0i where d == 0): fast Griffin-Lim's phase update"""
+    for t, nm in ((full, "full"), (mag, "mag"), (rebuilt, "rebuilt"), (prev, "prev")):
+        _f32c(t, f"gl_phase_momentum {nm}")
+    assert full.dtype == rebuilt.dtype == prev.dtype == torch.complex64 and mag.dtype == torch.float32
+    assert full.shape == rebuilt.shape == prev.shape == mag.shape
+    L.check(L.lib().taco_gl_phase_momentum(_p(full), _p(mag), _p(rebuilt), _p(prev), float(beta), mag.numel(), _st()),
+            "taco_gl_phase_momentum")
+
+
+def check_offsets(start, n, name="de_emphasis"):
+    """start int64 [S+1] (host): segment s = [start[s], start[s+1]) of a buffer of n samples, 0 <= start[0] and
+    non-decreasing up to start[S] <= n; raises ValueError naming the first entry that is not"""
+    s = np.asarray(start)
+    if s.ndim != 1 or s.size < 1 or s.dtype.kind not in "iu":
+        raise ValueError(f"{name}: start must be a 1-D integer array of S+1 offsets, got {s.dtype} {s.shape}")
+    s = s.astype(np.int64)
+    if s[0] < 0:
+        raise ValueError(f"{name}: start[0] = {int(s[0])} is negative")
+    down = np.flatnonzero(s[1:] < s[:-1])
+    if down.size:
+        i = int(down[0]) + 1
+        raise ValueError(f"{name}: start[{i}] = {int(s[i])} is below start[{i - 1}] = {int(s[i - 1])}")
+    if s[-1] > n:
+        raise ValueError(f"{name}: start[{s.size - 1}] = {int(s[-1])} is past the end of the {n}-sample buffer")
+    return s
+
+
+def de_emphasis(y, start, coef):
+    """in place: y[i] = x[i] + coef*y[i-1] over each segment [start[s], start[s+1]) of y (contiguous fp32), zero state
+    before start[s] (scipy.signal.lfilter([1], [1, -coef], .) per segment).  start (host, int64 [S+1]) is checked on the
+    host, then copied to the device: one launch."""
+    _cuda_c(y, torch.float32, "de_emphasis y")
+    s = check_offsets(start, y.numel())
+    if s.size - 1 > 2**31 - 1:
+        raise ValueError(f"de_emphasis: {s.size - 1} segments, at most 2^31 - 1 per launch")
+    start_d = torch.from_numpy(np.ascontiguousarray(s)).to(y.device)
+    L.check(L.lib().taco_de_emphasis(_p(y), _p(start_d), s.size - 1, float(coef), _st()), "taco_de_emphasis")
+
+
 def rfft2048(X, x):
     """X complex64 [..., 1025] = rfft(x fp32 [..., 2048]) over the last axis (unnormalised) -- librosa.stft's transform"""
     _f32c(X, "rfft2048 X"); _f32c(x, "rfft2048 x")

@@ -55,6 +55,16 @@ The WAV, the attention array and the summaries end at the stop (with ``--trim-ta
 that comes first; with ``--long-form`` a chunk whose rule fired is never split again).  It works with every other flag.
 The default hold of 4 steps is a starting point only: no value has been tried on a trained model here.  An utterance
 whose attention never reaches the end of its text decodes all ``max_decode_iter`` steps, as without the flag.
+
+    python -m tacotron_b200.test -t nancy --griffin-lim-momentum --griffin-lim-iters 25 --de-emphasis
+
+``--griffin-lim-iters N`` sets the Griffin-Lim iterations (default 50, the reference's).  ``--griffin-lim-momentum [M]``
+runs fast Griffin-Lim (Perraudin, Balazs & Sondergaard 2013), which adds a momentum term M in [0, 1] to the phase update
+(a bare flag: 0.99, librosa's default; default 0, plain Griffin-Lim).  ``--de-emphasis`` undoes preprocessing's
+pre-emphasis ``y[n] - 0.97 y[n-1]`` on every synthesised waveform with the inverse filter ``y[n] = x[n] + 0.97 y[n-1]``;
+with ``--long-form`` it runs once over each joined line, through its pauses and fades.  They work with every other flag,
+and without them every file is what the driver writes without them.  No value of either has been tried on a trained
+model here.
 """
 from __future__ import annotations
 
@@ -66,14 +76,18 @@ import numpy as np
 import torch
 
 
-def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, trim_tail=False, long_form=False):
+def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, trim_tail=False, long_form=False,
+         griffin_lim_iters=50, griffin_lim_momentum=0.0, de_emphasis=False):
     """summary_dir: also write each prompt's audio and attention image as TensorBoard summaries there, at step 0
     (tacotron_b200/summary.py).  trim_tail: end each utterance where its speech ends; long_form: speak each line as one
     clip, whatever its length (module docstring).  config.attention_window (None or (back, ahead)) and
-    config.stop_at_end (None or a hold) apply to every decode, plain and long-form.  Returns one device waveform per
-    prompt."""
+    config.stop_at_end (None or a hold) apply to every decode, plain and long-form.  griffin_lim_iters /
+    griffin_lim_momentum: the inversion's iterations and fast Griffin-Lim momentum; de_emphasis: undo preprocessing's
+    pre-emphasis on every waveform (module docstring).  Returns one device waveform per prompt."""
     from . import audio, checkpoint, data_input
     from .train import write_wav
+    gl = dict(n_iter=griffin_lim_iters, momentum=griffin_lim_momentum)
+    audio.gl_check(**gl)                                                                 # before any model is built
     sr = 24000 if "blizzard" in config.data_path else 16000                              # test.py:15
     meta = data_input.load_meta(config.data_path)                                        # :16
     config.r = meta["r"]          # (the reference reads the module constant audio.r here, :17; meta['r'] is the value it was preprocessed with)
@@ -116,7 +130,7 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, tri
     if long_form:
         try:
             return _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, sr, log, writer,
-                              scopes if writer is not None else None)
+                              scopes if writer is not None else None, gl, de_emphasis)
         finally:
             if writer is not None:
                 writer.close()
@@ -134,10 +148,15 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, tri
                 frames = audio.speech_frames(outputs, config.r, stft_mean=mean_d, stft_std=std_d) if trim_tail else None
                 if model.end_steps is not None:                                          # the stop rule's frames
                     frames = audio.stop_frames(model.end_steps, config.r, outputs.shape[1], frames)
-                wav = audio.invert_speech(outputs, config.r, frames, stft_mean=mean_d, stft_std=std_d)
+                y, start = audio.invert_speech_packed(outputs, config.r, frames, stft_mean=mean_d, stft_std=std_d, **gl)
+                if de_emphasis:
+                    audio.de_emphasis(y, start)
+                wav = [y[start[b]:start[b + 1]] for b in range(outputs.shape[0])]
                 steps = (frames.cpu() // config.r).tolist()
             else:
-                wav = audio.invert_spectrogram(outputs, config.r, stft_mean=mean_d, stft_std=std_d)   # :64, batched on the device
+                wav = audio.invert_spectrogram(outputs, config.r, stft_mean=mean_d, stft_std=std_d, **gl)   # :64, batched on the device
+                if de_emphasis:
+                    audio.de_emphasis(wav)
             for b in range(outputs.shape[0]):                                            # :59-70
                 text = "".join(ivocab[int(w)] for w in inputs["text"][b].cpu().numpy())
                 wave, alignment = wav[b].cpu().numpy(), alignments[b].cpu().numpy()
@@ -159,7 +178,7 @@ def test(model_cls, config, prompts, log=print, speaker=0, summary_dir=None, tri
     return waves
 
 
-def _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, sr, log, writer, scopes):
+def _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, sr, log, writer, scopes, gl, de_emphasis):
     """test(long_form=True): the rounds of synthesis and re-splitting, then the join (module docstring)"""
     from . import audio, data_input, longform
     from .train import write_wav
@@ -187,7 +206,7 @@ def _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, 
             bounds = bounds.cpu().numpy()    # the one read
             if bounds.shape[1] == 4:
                 bounds, fired = bounds[:, :3], bounds[:, 3] != 0
-            y, start = audio.invert_speech_packed(outputs, r, bounds[:, 2], stft_mean=mean_d, stft_std=std_d)
+            y, start = audio.invert_speech_packed(outputs, r, bounds[:, 2], stft_mean=mean_d, stft_std=std_d, **gl)
             align = model.alignments.cpu().numpy()
             n = 4 * r * (outputs.shape[1] // 4)
             outs.append(y)
@@ -222,6 +241,8 @@ def _long_form(model, config, prompts, ivocab, speaker, mean_d, std_d, out_dir, 
     out = torch.zeros(total, dtype=torch.float32, device=mean_d.device)
     for bi, rows in segs.items():
         audio.join_speech(out, outs[bi], np.asarray(rows, dtype=np.int64), sr)
+    if de_emphasis:                      # one segment per line: the filter runs through pauses and fades, not across lines
+        audio.de_emphasis(out, np.array([o for o, _ in spans] + [total], dtype=np.int64))
     waves = []
     for n, (cs, (o, length)) in enumerate(zip(lines, spans)):
         wave = out[o:o + length]
@@ -268,6 +289,28 @@ def parse_stop_hold(text):
     return hold
 
 
+def parse_gl_iters(text):
+    """'N' -> an int >= 0 (the --griffin-lim-iters value)"""
+    try:
+        n = int(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"{text!r}: expected N, an integer number of iterations such as 50") from None
+    if n < 0:
+        raise argparse.ArgumentTypeError(f"{text!r}: N must be >= 0")
+    return n
+
+
+def parse_gl_momentum(text):
+    """'M' -> a float in [0, 1] (the --griffin-lim-momentum value)"""
+    try:
+        m = float(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"{text!r}: expected M, a number in [0, 1] such as 0.99") from None
+    if not 0.0 <= m <= 1.0:
+        raise argparse.ArgumentTypeError(f"{text!r}: M must be in [0, 1]")
+    return m
+
+
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", "--train-set", default="nancy")
@@ -287,6 +330,13 @@ def main(argv=None):
     parser.add_argument("--stop-at-end", type=parse_stop_hold, nargs="?", const=4, default=None, metavar="HOLD",
                         help="stop decoding once HOLD consecutive steps attend to the last character of the text or "
                              "past it (a bare flag: 4, a starting point only)")
+    parser.add_argument("--griffin-lim-iters", type=parse_gl_iters, default=50, metavar="N",
+                        help="Griffin-Lim iterations (default 50, the reference's)")
+    parser.add_argument("--griffin-lim-momentum", type=parse_gl_momentum, nargs="?", const=0.99, default=0.0, metavar="M",
+                        help="fast Griffin-Lim with momentum M in [0, 1] (a bare flag: 0.99, librosa's default; "
+                             "default 0, the reference's plain Griffin-Lim)")
+    parser.add_argument("--de-emphasis", action="store_true",
+                        help="undo preprocessing's pre-emphasis (y[n] - 0.97 y[n-1]) on every synthesised waveform")
     args = parser.parse_args(argv)
     prompts = [p for p in sys.stdin.readlines() if len(p) > 0]                           # test.py:77-78
     from .models.tacotron import Config, Tacotron
@@ -299,7 +349,8 @@ def main(argv=None):
     print("Building Tacotron")
     summary_dir = os.path.join("log", config.save_path, "test") if args.summaries else None      # test.py:33
     test(Tacotron, config, prompts, speaker=args.speaker, summary_dir=summary_dir, trim_tail=args.trim_tail,
-         long_form=args.long_form)
+         long_form=args.long_form, griffin_lim_iters=args.griffin_lim_iters,
+         griffin_lim_momentum=args.griffin_lim_momentum, de_emphasis=args.de_emphasis)
 
 
 if __name__ == "__main__":
